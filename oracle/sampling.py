@@ -163,10 +163,15 @@ def mipmap_levels(grid, height, width, max_num_levels, min_level=0.0):
     return torch.log2(d).clamp(min=0.0, max=max_num_levels - 1.0).clamp(min=min_level)
 
 
-def mipmap_warp_ref(x, grid, max_num_levels=8, min_level=0.0, padding_mode="border", return_aux=False):
-    """MipmapWarp.forward (:35-60).  Returns out [, dict(levels, level_0, level_1, num_levels, levels_map)]."""
+def mipmap_warp_ref(x, grid, max_num_levels=8, min_level=0.0, padding_mode="border", return_aux=False,
+                    detach_levels=False):
+    """MipmapWarp.forward (:35-60).  Returns out [, dict(levels, level_0, level_1, num_levels, levels_map)].
+    `detach_levels`: no gradient through the level of detail, so d out / d grid is the bilinear part alone; its
+    difference from the default (levels live, as in the reference) is the level-of-detail part."""
     n, c, h, w = x.shape
     levels = mipmap_levels(grid, h, w, max_num_levels, min_level)
+    if detach_levels:
+        levels = levels.detach()
     num_levels = int(levels.max().ceil().item()) + 1                      # :52 (batch-global, host sync)
     stack = create_stack(x, num_levels)                                   # (N, C, D, H, W)
     d = stack.shape[2]

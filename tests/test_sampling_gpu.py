@@ -15,6 +15,137 @@ def _stn():
     return stn
 
 
+# out / grad_x vs the float64 oracle, relative to the largest entry.  fp32: the source coordinate ((g + 1) * size - 1) / 2
+# rounds at ulp(2) * size / 2 (6e-5 px on a 512 px source), which a random image's slopes of a few units per px turn into
+# ~1e-4 of the output's magnitude; half precision: the output is rounded to the source's type.
+LOW_PRECISION_TOL = {torch.float32: 3e-4, torch.float16: 1e-3, torch.bfloat16: 8e-3}
+
+
+def level_atol(size):
+    """levels vs the float64 oracle: the level of detail is log2 of a difference of fp32 coordinates of up to ~size px,
+    which cancellation leaves with ~ulp(coordinate) / distance relative error: measured 3e-5 (128 px source) and 1.6e-4
+    (512 px) in log2 units at 1-2 px distances."""
+    return 1e-4 * max(1.0, size / 200.0)
+
+
+# ------------------------------------------------------------------------------------------------ "decided" pixels
+# The sampler makes discrete choices: the bilinear corner floor(c), the mip levels floor / ceil(level), the arg-max
+# neighbour of the level of detail and the clamps of both.  Where the oracle's value sits within rounding noise of such a
+# boundary, the last ulp of the fp32 evaluation order decides the choice (on the GPU as in ATen's own CUDA kernel), and the
+# grid gradient jumps there.  Those pixels are exempt from the grid-gradient comparisons; the exempt set must stay tiny.
+# The level thresholds are those of the fp32 level of detail (level_atol): level_atol of a level, half of it relative
+# between the two largest neighbour distances.
+def coordinate_decided(c, size, mode, exact_integers=False):
+    """floor(c) is decided: c is not within 1e-4 px of an integer -- or pinned to a border pixel by the clamp of the border /
+    reflection modes (an exact constant on both sides).  `exact_integers`: c is the float64 image of fp32 arithmetic that is
+    exact on both sides (dyadic grids; float64 of fp32 inputs, where an exact integer is an exact integer in fp32 too)."""
+    off = (c - c.round()).abs()
+    ok = off > 1e-4
+    if exact_integers:
+        ok |= off == 0
+    if mode != "zeros":
+        ok |= (c == 0) | (c == size - 1)
+    return ok
+
+
+def level_decided(lv):
+    """floor / ceil of a level of detail are decided: not within 1e-5 of an integer -- or exactly 0, the clamp of a
+    distance <= 1 px (an exact constant on both sides)."""
+    return ((lv - lv.round()).abs() > 1e-5) | (lv == 0)
+
+
+def neighbour_sq(grid, hs, ws):
+    """(4, N, Ho, Wo) squared distances, in level-of-detail coordinates, to the left / right / up / down neighbour
+    (replicate-clamped at the image border), unclamped -- the oracle's max_coord_distance before its clamp(min=1)."""
+    c = S.lod_coordinates(grid, hs, ws)
+    p = F.pad(c.permute(0, 3, 1, 2), (1, 1, 1, 1), mode="replicate").permute(0, 2, 3, 1)
+    neigh = [p[:, 1:-1, :-2], p[:, 1:-1, 2:], p[:, :-2, 1:-1], p[:, 2:, 1:-1]]
+    return torch.stack([((o - c) ** 2).sum(dim=3) for o in neigh])
+
+
+def _mark_targets(bad, nb_idx, sel):
+    """bad |= the neighbours nb_idx (0 left, 1 right, 2 up, 3 down; replicate-clamped) of the pixels `sel`."""
+    n, ho, wo = bad.shape
+    ni, yi, xi = torch.meshgrid(torch.arange(n), torch.arange(ho), torch.arange(wo), indexing="ij")
+    ty = (yi + torch.tensor([0, 0, -1, 1])[nb_idx]).clamp(0, ho - 1)
+    tx = (xi + torch.tensor([-1, 1, 0, 0])[nb_idx]).clamp(0, wo - 1)
+    bad[ni[sel], ty[sel], tx[sel]] = True
+
+
+def undecided_pixels(grid, hs, ws, mode, max_level=None, min_level=0.0, grid_gradient=True):
+    """(N, Ho, Wo) bool, from the float64 grid: a bilinear coordinate within 1e-4 px of an integer, or (mip sampling,
+    `max_level` not None) the level within level_atol of an integer or of a clamp, or the top two neighbour distances within
+    half of that relative, or (border / reflection) the coordinate within 1e-4 px of the clip.  Exactly-on values are
+    decided: the float64 images of fp32 inputs are exact, and so are their ties.
+    `grid_gradient`: a pixel also receives the level-of-detail term of every neighbour that targets it, so an undecided
+    level or arg-max also marks every neighbour that may be the arg-max (a corner index only moves the
+    pixel's own terms: the level-of-detail term is continuous in it)."""
+    g = grid.double()
+    bad = torch.zeros(g.shape[:3], dtype=torch.bool)
+    for k, size in ((0, ws), (1, hs)):
+        bad |= ~coordinate_decided(S.source_index(g[..., k], size, mode), size, mode, True)
+        if mode != "zeros":     # the clip itself: a coordinate at the border is clamped (gradient 0) on one side only
+            raw = ((g[..., k] + 1.0) * size - 1.0) / 2.0
+            raw = S._reflect(raw, -1, 2 * size - 1) if mode == "reflection" else raw
+            for edge in (0.0, size - 1.0):
+                bad |= ((raw - edge).abs() <= 1e-4) & (raw != edge)
+    if max_level is None:
+        return bad
+    sq = neighbour_sq(g, hs, ws)
+    raw = 0.5 * torch.log2(sq.max(dim=0).values)          # unclamped level; -inf where every neighbour coincides
+    off = (raw - raw.round()).abs()
+    tol = level_atol(max(hs, ws))
+    level_bad = (off > 0) & (off <= tol) & (raw >= -tol) & (raw <= max_level + tol)
+    for clamp in (max_level, min_level):
+        level_bad |= (raw != clamp) & ((raw - clamp).abs() <= tol)
+    top = sq.clamp(min=1.0).sqrt().topk(2, dim=0)
+    gap = top.values[0] - top.values[1]
+    tie_bad = (gap > 0) & (gap <= 0.5 * tol * top.values[0])
+    bad |= level_bad | tie_bad
+    if grid_gradient:
+        # the kernel's arg-max may be ANY neighbour whose distance lies within the rounding band of the largest (three of them
+        # can be that close), judged by the UNCLAMPED distance: below 1 px the clamp ties them all, the rounding does not
+        band = sq >= sq.max(dim=0).values * (1.0 - tol)
+        for k in range(4):
+            _mark_targets(bad, torch.full(bad.shape, k), (level_bad | tie_bad) & band[k])
+    return bad
+
+
+def warp_oracle(x, grid, go, num_levels, min_level, mode):
+    """float64 autograd of the oracle on the kernel's inputs (x, grid, go as the kernel sees them) ->
+    out, levels, grad_x, grad_grid, and grad_grid with the levels detached (the bilinear part alone)."""
+    xd = x.double().requires_grad_(True)
+    gd = grid.double().requires_grad_(True)
+    out, aux = S.mipmap_warp_ref(xd, gd, num_levels, min_level, mode, return_aux=True)
+    gx, gg = torch.autograd.grad(out, [xd, gd], go.double())
+    gd2 = grid.double().requires_grad_(True)
+    (gg_det,) = torch.autograd.grad(S.mipmap_warp_ref(x.double(), gd2, num_levels, min_level, mode, detach_levels=True),
+                                    gd2, go.double())
+    return out.detach(), aux["levels"], gx, gg, gg_det
+
+
+def check_grid_grad(gg, gg_o, gg_det, exempt, rtol, lod_rtol, what, need_lod=True):
+    """The kernel's grid gradient vs the float64 oracle on the decided pixels (tolerance relative to its largest entry);
+    then its level-of-detail share alone -- kernel minus the oracle with levels detached, vs the oracle's live minus
+    detached -- on THAT share's own scale, over the whole grid and over the pixels of the four output borders (where the
+    neighbour gather meets the clamps), so that an error in a term much smaller than the bilinear part still shows."""
+    gg = gg.detach().double().cpu()
+    keep = ~exempt[..., None].expand_as(gg)
+    assert_close(gg[keep], gg_o[keep], rtol=rtol, what=what + " grad_grid")
+    lod_o, lod_k = gg_o - gg_det, gg - gg_det
+    if need_lod:
+        assert lod_o[keep].abs().max() > 0, what + ": no level-of-detail gradient to check"
+    if lod_o[keep].abs().max() == 0:     # every level clamped: the share is zero, and the check above covers the rest
+        return
+    assert_close(lod_k[keep], lod_o[keep], rtol=lod_rtol, what=what + " level-of-detail share")
+    border = torch.zeros(exempt.shape, dtype=torch.bool)
+    border[:, 0] = border[:, -1] = True
+    border[:, :, 0] = border[:, :, -1] = True
+    keep_b = keep & border[..., None]
+    if lod_o[keep_b].abs().max() > 0:
+        assert_close(lod_k[keep_b], lod_o[keep_b], rtol=lod_rtol, what=what + " level-of-detail share at the borders")
+
+
 def test_mipmap_warp_golden_forward_backward_and_levels():
     stn = _stn()
     blob = load_golden("mipmap_warp")
@@ -48,19 +179,135 @@ def test_mipmap_warp_golden_forward_backward_and_levels():
 @pytest.mark.parametrize("size,res,mode", [(128, 128, "border"), (256, 128, "reflection"), (450, 128, "border"),
                                            (512, 512, "border"), (64, 96, "zeros")])
 def test_mipmap_warp_vs_oracle_training_shapes(size, res, mode):
+    """Forward, levels, grad_x (scatter + pyramid adjoint) and grad_grid (bilinear part + the level-of-detail gather) vs
+    float64 autograd of the oracle at the STN's shapes."""
+    _check_training_shape(size, res, mode, torch.float32)
+
+
+@pytest.mark.parametrize("size,res,mode,dtype", [(256, 128, "reflection", torch.float16), (450, 128, "border", torch.bfloat16),
+                                                 (64, 96, "zeros", torch.float16), (128, 128, "border", torch.bfloat16)])
+def test_mipmap_warp_vs_oracle_half_precision_sources(size, res, mode, dtype):
+    """The same with fp16 / bf16 sources: the oracle gets the same rounded source and output gradient (the kernel reads them
+    as they are and computes in fp32); out and grad_x are rounded to the source's type, grad_grid is fp32."""
+    _check_training_shape(size, res, mode, dtype)
+
+
+def _check_training_shape(size, res, mode, dtype):
     stn = _stn()
     g = torch.Generator().manual_seed(size + res)
     n = 3
-    x = torch.randn(n, 3, size, size, generator=g)
+    x = torch.randn(n, 3, size, size, generator=g).to(dtype)
     theta = torch.tensor([[1.0, 0.0, 0.0, 0.0, 1.0, 0.0], [1.9, 0.6, 0.1, -0.6, 1.9, -0.1], [3.0, 0.0, 0.2, 0.0, 3.0, 0.0]]).reshape(3, 2, 3)
     coarse = torch.randn(n, 2, 6, 6, generator=g)
     grid = F.affine_grid(theta, (n, 3, res, res), align_corners=False) + \
         0.08 * F.interpolate(coarse, size=(res, res), mode="bicubic", align_corners=False).permute(0, 2, 3, 1)
-    yo, aux = S.mipmap_warp_ref(x, grid, 3.5, 0.0, mode, return_aux=True)
+    go = torch.randn(n, 3, res, res, generator=g).to(dtype)
+    yo, lv_o, gx_o, gg_o, gg_det = warp_oracle(x, grid, go, 3.5, 0.0, mode)
     mw = stn.MipmapWarp(3.5).to(DEV)
-    y = mw(x.to(DEV), grid.to(DEV), padding_mode=mode)
-    assert_close(y, yo, rtol=1e-4, what="fwd")
-    assert_close(mw.levels_map.cpu() * 2.5, aux["levels"], atol=5e-6, what="levels")
+    xg, gr = x.to(DEV).requires_grad_(True), grid.to(DEV).requires_grad_(True)
+    y = mw(xg, gr, padding_mode=mode)
+    assert y.dtype == dtype
+    tol = LOW_PRECISION_TOL[dtype]
+    assert_close(y, yo, rtol=tol, what="fwd")
+    assert_close(mw.levels_map.cpu() * 2.5, lv_o, atol=level_atol(size), what="levels")
+    gx, gg = torch.autograd.grad(y, [xg, gr], go.to(DEV))
+    assert gx.dtype == dtype and gg.dtype == torch.float32
+    assert_close(gx, gx_o, rtol=tol, what="grad_x")
+    exempt = undecided_pixels(grid, size, size, mode, 2.5)
+    # these grids are affine plus a smooth perturbation: a pixel's left and right (up and down) distances differ only by the
+    # perturbation's second difference, so 1-2 % of the pixels hold their top distances within the rounding of the fp32
+    # level-of-detail coordinates (5 % on the 512 px source, whose coordinates are larger)
+    assert exempt.float().mean() < (0.06 if size >= 512 else 0.03)
+    check_grid_grad(gg, gg_o, gg_det, exempt, GRID_RTOL, LOD_RTOL, "%d->%d %s" % (size, res, mode))
+
+
+# grid-gradient tolerances, relative to the largest entry of the whole gradient / of its level-of-detail share
+GRID_RTOL, LOD_RTOL = 1e-4, 1e-4
+
+
+def _dyadic(k):
+    return k.double() / 512.0
+
+
+def _edge_grid(case):
+    """Constructed grids (N, Ho, Wo, 2), source size and sampler settings for the edges of the grid-gradient gather."""
+    yy, xx = torch.meshgrid(torch.arange(16), torch.arange(16), indexing="ij")
+    if case == "pinch":
+        # a zoomed-out dyadic affine grid (~4 px between neighbours) with three points displaced ~20 px: every neighbour of
+        # the displaced interior point (4), edge point (3) and corner point (2) takes it as its arg-max neighbour
+        k = torch.stack([64 * xx + 9 * yy - 540, -6 * xx + 60 * yy - 480], dim=-1)
+        for y, x in ((8, 8), (0, 5), (15, 15)):
+            k[y, x] += torch.tensor([256, -205])
+        return _dyadic(k[None]).float(), 64, 8, 0.0
+    if case == "ties":
+        # dyadic affine grid (k/512): left/right and up/down distances tie EXACTLY (in fp32 too), half the pixels nudged by
+        # +-1/512 so that some ties break; "first maximum, order left, right, up, down" = torch.max(dim=0)'s first index
+        g = torch.Generator().manual_seed(5)
+        kx = 40 * xx + 13 * yy - 300
+        ky = -11 * xx + 37 * yy - 280
+        k = torch.stack([kx, ky], dim=-1) + torch.randint(-1, 2, (16, 16, 2), generator=g) * (torch.rand(16, 16, 1, generator=g) < 0.5)
+        return _dyadic(k[None]).float(), 64, 8, 0.0
+    if case.startswith("clamps"):
+        # 65 px source: level-of-detail coordinates are k/16 + 32, so steps of 16, 24, 32, 48, 64, 128 (/512) are distances
+        # of exactly 1 (sq == 1: level 0 at the clamp), 1.5, 2, 3, 4 (level 2 = min_level of "clamps_min") and 8 px
+        # (level 3 = max_level); a corner patch has unit steps only, the
+        # crossing of rows and columns 10..13 4 px steps only
+        g = torch.Generator().manual_seed(6)
+        steps = torch.tensor([16, 24, 32, 48, 64, 128])
+        sx, sy = steps[torch.randint(0, 6, (16, 16), generator=g)], steps[torch.randint(0, 6, (16, 16), generator=g)]
+        sx[:4, :4] = sy[:4, :4] = 16
+        sx[10:14, :] = 64
+        sy[:, 10:14] = 64
+        kx, ky = sx.cumsum(1), sy.cumsum(0)
+        k = torch.stack([kx - kx[8, 8], ky - ky[8, 8]], dim=-1)
+        return _dyadic(k[None]).float(), 65, 4, (2.0 if case == "clamps_min" else 0.0)
+    # "borders": source coordinates exactly on (and just inside / outside of) both borders: k = -504 / 504 is c = 0 / 63
+    # on a 64 px source, k = -512 / 512 the edges of the normalised range (reflection folds them onto the borders)
+    kx = torch.where(xx < 8, -528 + 4 * xx, 488 + 4 * (xx - 8))
+    ky = -504 + 84 * yy
+    return _dyadic(torch.stack([kx, ky], dim=-1)[None]).float(), 64, 8, 0.0
+
+
+@pytest.mark.parametrize("mode", S.PAD_MODES)
+@pytest.mark.parametrize("case", ["pinch", "ties", "clamps", "clamps_min", "borders"])
+def test_mipmap_warp_grid_gradient_edges(case, mode):
+    """The gathered grid gradient (csrc/warp.cu warp_bwd_kernel) on constructed grids: one target shared by 2, 3 and 4
+    neighbours, exact arg-max ties, distances and levels exactly at their clamps, source coordinates exactly on the
+    borders -- vs float64 autograd of the oracle, with its level-of-detail share checked on its own scale."""
+    stn = _stn()
+    grid, size, num_levels, min_level = _edge_grid(case)
+    g = torch.Generator().manual_seed(7)
+    n, ho, wo = grid.shape[:3]
+    x = torch.randn(n, 3, size, size, generator=g)
+    go = torch.randn(n, 3, ho, wo, generator=g)
+    max_level = min(num_levels - 1.0, float(stn.sampling.feasible_levels(size, size, num_levels - 1)))
+    sq = neighbour_sq(grid.double(), size, size)
+    arg = sq.clamp(min=1.0).sqrt().max(dim=0).indices[0]
+    if case == "pinch":
+        # how many neighbours pick each pixel as their arg-max target
+        ty = (torch.arange(ho)[:, None] + torch.tensor([0, 0, -1, 1])[arg]).clamp(0, ho - 1)
+        tx = (torch.arange(wo)[None, :] + torch.tensor([-1, 1, 0, 0])[arg]).clamp(0, wo - 1)
+        hits = torch.zeros(ho, wo, dtype=torch.long).index_put_((ty.flatten(), tx.flatten()), torch.ones(ho * wo, dtype=torch.long),
+                                                                accumulate=True)
+        assert hits[8, 8] == 4 and hits[0, 5] == 3 and hits[15, 15] == 2
+    if case != "pinch":
+        top = sq.clamp(min=1.0).sqrt().topk(2, dim=0).values
+        assert ((top[0] == top[1]) & (top[0] > 1)).sum() >= 3           # exact ties with a live gradient
+    if case.startswith("clamps"):
+        sq_max = sq.max(dim=0).values
+        assert (sq_max == 1).any() and (sq_max == 64).any() and (sq_max == 16).any()
+    yo, lv_o, gx_o, gg_o, gg_det = warp_oracle(x, grid, go, num_levels, min_level, mode)
+    mw = stn.MipmapWarp(num_levels).to(DEV)
+    xg, gr = x.to(DEV).requires_grad_(True), grid.to(DEV).requires_grad_(True)
+    y = mw(xg, gr, min_level=min_level, padding_mode=mode)
+    assert_close(y, yo, rtol=LOW_PRECISION_TOL[torch.float32], what="fwd")
+    assert_close(mw.levels_map.cpu() * (num_levels - 1.0), lv_o, atol=level_atol(size), what="levels")
+    gx, gg = torch.autograd.grad(y, [xg, gr], go.to(DEV))
+    assert_close(gx, gx_o, rtol=1e-4, what="grad_x")
+    exempt = undecided_pixels(grid, size, size, mode, max_level, min_level)
+    # the dyadic grids are exact in fp32: every pixel is decided, ties and clamps included
+    assert exempt.sum() == 0
+    check_grid_grad(gg, gg_o, gg_det, exempt, GRID_RTOL, LOD_RTOL, "%s %s" % (case, mode))
 
 
 def test_mipmap_warp_min_level_and_warp_match_torch_grid_sample():
@@ -170,17 +417,172 @@ def test_sampler_integer_work_is_bit_exact(mode, hs, ws):
         if name == "dyadic":
             corner_ok = torch.ones_like(x0, dtype=torch.bool)
         else:
-            def decided(c, size):      # not within 1e-4 px of an integer -- or pinned to a border pixel by the clamp of the
-                ok = (c - c.round()).abs() > 1e-4                      # border / reflection modes (an exact constant on both sides)
-                if mode != "zeros":
-                    ok |= (c == 0) | (c == size - 1)
-                return ok
-            corner_ok = decided(ix, ws) & decided(iy, hs)
+            corner_ok = coordinate_decided(ix, ws, mode) & coordinate_decided(iy, hs, mode)
             assert corner_ok.float().mean() > 0.995
         assert torch.equal(got[..., 0][corner_ok].long(), x0[corner_ok]), name + " x0"
         assert torch.equal(got[..., 1][corner_ok].long(), y0[corner_ok]), name + " y0"
-        level_ok = (lv - lv.round()).abs() > 1e-5
-        level_ok |= lv == 0                                 # the clamp: distance <= 1 px is level 0 exactly on both sides
+        level_ok = level_decided(lv)
         assert level_ok.float().mean() > 0.995
         assert torch.equal(got[..., 2][level_ok].long(), lv.floor().long()[level_ok]), name + " floor(level)"
         assert torch.equal(got[..., 3][level_ok].long(), lv.ceil().long()[level_ok]), name + " ceil(level)"
+
+
+# ------------------------------------------------------------------------------------------------ one-pass STN sampler
+def grid_stride_batch(ho, wo):
+    """A batch whose N * Ho * Wo output pixels exceed one trip of the sampler's grid-stride loops (16 CTAs of 256 threads
+    per SM: csrc/warp.cu grid_for, csrc/flow.cu flow_grid), so that every thread makes a second trip."""
+    from gangealing_b200 import _lib
+    return _lib.sm_count() * 16 * 256 // (ho * wo) + 2
+
+
+def _kernel_grid_grad(x, grid, go, levels, mode):
+    """The sampler's own backward (the kernel stn_sample_* call) on a given grid: its gradient w.r.t. the grid."""
+    from gangealing_b200.stn import sampling as GS
+    gk = grid.detach().requires_grad_(True)
+    if levels is None:
+        y = GS.grid_sample_bilinear(x, gk, mode)
+    else:
+        y = GS.mipmap_warp(x, gk, levels, 0.0, mode)[0]
+    return torch.autograd.grad(y, gk, go)[0].double().cpu()
+
+
+def _sampler_oracle(x, grid, go, levels, mode, hs, ws, affine):
+    """The sampling stage of stn_sample_* on the grid the kernel generated (`grid`, returned by it; checked against the
+    oracle's generator by the caller) -> float64 oracle out, levels, grad_x, and the kernel's own per-pixel grid gradient
+    (its sampler backward on that grid), checked per pixel against the oracle's on the decided pixels.  The caller checks
+    the grid generator's backward against float64 autograd of the oracle's generator fed with THAT gradient: a sum over
+    pixels (g_theta, g_base, g_low) would otherwise inherit the O(1) jumps of the few undecided pixels.
+    `affine` with levels: an affine grid has equal left / right (and up / down) neighbour distances at every pixel, so
+    rounding picks the level-of-detail arg-max everywhere and no pixel is decided; the per-pixel grid gradient is left to the
+    MipmapWarp tests above (non-affine grids, and exact ties on dyadic grids).  g_theta does not depend on that choice."""
+    xd = x.double().requires_grad_(True)
+    gl = grid.detach().double().cpu().requires_grad_(True)
+    if levels is None:
+        out, lv, gg_det = S.warp_ref(xd, gl, mode), None, None
+    else:
+        out, aux = S.mipmap_warp_ref(xd, gl, levels, 0.0, mode, return_aux=True)
+        lv = aux["levels"]
+        gd2 = gl.detach().clone().requires_grad_(True)
+        (gg_det,) = torch.autograd.grad(S.mipmap_warp_ref(x.double(), gd2, levels, 0.0, mode, detach_levels=True), gd2, go.double())
+    gx, gg = torch.autograd.grad(out, [xd, gl], go.double())
+    gg_k = _kernel_grid_grad(x.to(DEV), grid, go.to(DEV), levels, mode)
+    if not (affine and levels is not None):
+        exempt = undecided_pixels(gl.detach(), hs, ws, mode, None if levels is None else levels - 1.0)
+        assert exempt.float().mean() < 0.005
+        if levels is None:
+            keep = ~exempt[..., None].expand_as(gg)
+            assert_close(gg_k[keep], gg[keep], rtol=GRID_RTOL, what="sampler grid gradient")
+        else:
+            check_grid_grad(gg_k, gg, gg_det, exempt, GRID_RTOL, LOD_RTOL, "sampler", need_lod=False)
+    return out.detach(), lv, gx, gg_k
+
+
+def _check_stn_affine(n, out_hw, levels, mode, dtype, seed=0):
+    from gangealing_b200.stn import sampling as GS
+    g = torch.Generator().manual_seed(seed + out_hw[0] * 1000 + out_hw[1])
+    hs = ws = 128
+    ho, wo = out_hw
+    x = torch.randn(n, 3, hs, ws, generator=g).to(dtype)
+    # zoom in and out, rotation / shear, translation
+    theta = torch.eye(2, 3)[None] * (0.5 + 1.5 * torch.rand(n, 1, 1, generator=g)) + 0.15 * torch.randn(n, 2, 3, generator=g)
+    go = torch.randn(n, 3, ho, wo, generator=g).to(dtype)
+    g_grid = torch.randn(n, ho, wo, 2, generator=g)          # the caller also uses the returned grid
+    x_dev, go_dev = x.to(DEV), go.to(DEV)
+    xg, tg = x_dev.clone().requires_grad_(True), theta.to(DEV).requires_grad_(True)
+    out, grid, lv = GS.stn_sample_affine(xg, tg, out_hw, levels, 0.0, mode)
+    gx, gth = torch.autograd.grad((out.float() * go_dev.float()).sum() + (grid * g_grid.to(DEV)).sum(), [xg, tg])
+    # oracle
+    th = theta.double().requires_grad_(True)
+    grid_o = S.affine_grid_ref(th, (n, 3, ho, wo))
+    assert_close(grid, grid_o, rtol=1e-6, what="grid")
+    out_o, lv_o, gx_o, gg_k = _sampler_oracle(x, grid, go, levels, mode, hs, ws, affine=True)
+    tol = LOW_PRECISION_TOL[dtype]
+    assert out.dtype == dtype and gx.dtype == dtype
+    assert_close(out, out_o, rtol=tol, what="out")
+    if levels is None:
+        assert lv is None
+    else:
+        assert_close(lv, lv_o, atol=level_atol(hs), what="levels")
+    assert_close(gx, gx_o, rtol=tol, what="grad_x")
+    (gth_o,) = torch.autograd.grad(grid_o, th, gg_k + g_grid.double())
+    assert_close(gth, gth_o, rtol=1e-4, what="g_theta")
+
+
+@pytest.mark.parametrize("mode", S.PAD_MODES)
+@pytest.mark.parametrize("levels", [None, 4])
+@pytest.mark.parametrize("out_hw", [(128, 128), (100, 60), (7, 300), (1, 1)])
+def test_stn_sample_affine_vs_oracle(out_hw, levels, mode):
+    """The one-pass sampler (csrc/warp.cu warp_compose_fwd_kernel: affine grid generated in 32x8 tiles with a clamped halo)
+    and its hand-written backward (stn/sampling.py _StnSample) vs affine_grid_ref + mipmap_warp_ref in float64: out, the
+    returned grid and levels, grad_x and g_theta.  Output sizes: training, tiles overhanging the image, a single pixel
+    (every neighbour clamps onto itself)."""
+    _check_stn_affine(3, out_hw, levels, mode, torch.float32)
+
+
+FLOW_CASES = [  # low h, w, s, base warp, alpha, max_num_levels, padding mode
+    (16, 16, 8, True, None, 4, "border"), (16, 16, 8, False, "n", 4, "reflection"), (16, 16, 8, True, "1", None, "zeros"),
+    (12, 20, 4, True, "1", 4, "zeros"), (12, 20, 4, False, None, None, "border"), (12, 20, 4, True, "n", 4, "reflection"),
+    (7, 9, 1, True, "n", 4, "reflection"), (7, 9, 1, False, "1", None, "zeros"), (7, 9, 1, False, None, 4, "border")]
+
+
+def _check_stn_flow(n, lh, lw, s, with_base, alpha_kind, levels, mode, dtype, seed=0):
+    from gangealing_b200.stn import sampling as GS
+    from oracle import flow as FL
+    g = torch.Generator().manual_seed(seed + lh * 100 + lw + s)
+    ho, wo = lh * s, lw * s
+    hs = ws = 128 if s > 1 else 32
+    x = torch.randn(n, 3, hs, ws, generator=g).to(dtype)
+    low = (0.1 / s) * torch.randn(n, lh, lw, 2, generator=g)
+    mask = 2.0 * torch.randn(n, 9 * s * s, lh, lw, generator=g)
+    base = (torch.eye(2, 3)[None] * 1.4 + 0.1 * torch.randn(n, 2, 3, generator=g)) if with_base else None
+    alpha = {None: None, "n": torch.rand(n, generator=g), "1": torch.rand(1, generator=g)}[alpha_kind]
+    ident = S.affine_grid_ref(torch.eye(2, 3)[None], (1, 1, ho, wo))
+    go = torch.randn(n, 3, ho, wo, generator=g).to(dtype)
+    g_flow, g_delta = torch.randn(n, ho, wo, 2, generator=g), torch.randn(n, ho, wo, 2, generator=g)   # the TV loss's use
+    x_dev, go_dev = x.to(DEV), go.to(DEV)
+    leaves = [t.to(DEV).requires_grad_(True) for t in ([low, mask] + ([base] if with_base else []))]
+    out, flow, delta, lv = GS.stn_sample_flow(x_dev, leaves[0], leaves[1], ident.to(DEV), leaves[2] if with_base else None,
+                                              None if alpha is None else alpha.to(DEV), s, levels, 0.0, mode)
+    loss = (out.float() * go_dev.float()).sum() + (flow * g_flow.to(DEV)).sum() + (delta * g_delta.to(DEV)).sum()
+    grads = torch.autograd.grad(loss, leaves)
+    # oracle
+    leaves_o = [t.double().requires_grad_(True) for t in ([low, mask] + ([base] if with_base else []))]
+    delta_o, flow_o = FL.flow_compose_ref(leaves_o[0], leaves_o[1], ident.double(), leaves_o[2] if with_base else None,
+                                          None if alpha is None else alpha.double(), s)
+    assert_close(delta, delta_o, rtol=1e-5, what="delta")
+    assert_close(flow, flow_o, rtol=1e-5, what="flow")
+    out_o, lv_o, _, gg_k = _sampler_oracle(x, flow, go, levels, mode, hs, ws, affine=False)
+    assert out.dtype == dtype
+    assert_close(out, out_o, rtol=LOW_PRECISION_TOL[dtype], what="out")
+    if levels is None:
+        assert lv is None
+    else:
+        assert_close(lv, lv_o, atol=level_atol(hs), what="levels")
+    grads_o = torch.autograd.grad([flow_o, delta_o], leaves_o, [gg_k + g_flow.double(), g_delta.double()])
+    for a, e, nm in zip(grads, grads_o, ("g_low", "g_mask", "g_base")):
+        assert_close(a, e, rtol=1e-4, what=nm)
+
+
+@pytest.mark.parametrize("lh,lw,s,with_base,alpha,levels,mode", FLOW_CASES)
+def test_stn_sample_flow_vs_oracle(lh, lw, s, with_base, alpha, levels, mode):
+    """The one-pass flow sampler (RAFT convex up-sampling + identity + base warp + alpha generated inside the sampler) and
+    its backward (sampler backward, then csrc/flow.cu) vs flow_compose_ref + mipmap_warp_ref in float64, with a loss that
+    also uses the returned flow and delta (as the TV loss does): out, flow, delta, levels, g_low, g_mask, g_base.
+    Low-res sizes: training (16x16, s=8), non-square with 80 columns (not a multiple of the 32-wide tile), s=1."""
+    _check_stn_flow(3, lh, lw, s, with_base, alpha, levels, mode, torch.float32)
+
+
+@pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
+def test_stn_sample_low_precision_sources(dtype):
+    """Half-precision sources: the kernels read them as they are and compute in fp32; the oracle gets the same rounded
+    source and output gradient, so g_theta / g_low / g_mask / g_base keep the fp32 bound and only `out` is rounded."""
+    _check_stn_affine(3, (128, 128), 4, "border", dtype)
+    _check_stn_flow(3, 16, 16, 8, True, "n", 4, "reflection", dtype)
+
+
+def test_stn_sample_beyond_the_grid_stride_cap():
+    """Batch-32-and-up sampling at 128^2: more output pixels than the capped grids have threads, so the backward kernels
+    (warp_bwd_kernel, flow_compose_bwd_kernel) make a second trip through their grid-stride loops."""
+    n = grid_stride_batch(128, 128)
+    _check_stn_affine(n, (128, 128), 4, "border", torch.float32, seed=1)
+    _check_stn_flow(n, 16, 16, 8, True, "n", 4, "border", torch.float32, seed=1)

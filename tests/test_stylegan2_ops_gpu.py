@@ -5,6 +5,7 @@ import torch
 
 from conftest import assert_close, golden_cases, load_golden
 from oracle import stylegan2_ops as so
+from test_demod_precision import DEMOD_CASES, DEMOD_RTOL, demod_inputs, demod_ref, max_rel_err
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -353,3 +354,69 @@ def test_noise_bias_act_with_row_scale():
     gx, grs = torch.autograd.grad(y, [xg, rsg], go.to(DEV))
     assert_close(gx, go_x, rtol=1e-5, what="gx")
     assert_close(grs, go_rs, rtol=1e-4, what="g row_scale")
+
+
+# ------------------------------------------------------------------------------------------------ demodulation coefficients
+# the 13 demodulated convolutions of the 256^2 generator (channel multiplier 2) as (O, I): conv1 at 4^2, then an up-sampling
+# and a plain convolution per resolution 8^2 .. 256^2
+GEN256_DEMOD_LAYERS = [(512, 512)] * 9 + [(256, 512), (256, 256), (128, 256), (128, 128)]
+
+
+def _demod_style_grad_ref(w, s, scale, gd, eps=1e-8):
+    """float64 autograd of demod_ref w.r.t. the style, and the same contraction over |terms| (the scale of its rounding)."""
+    sd = s.double().requires_grad_(True)
+    (gs,) = torch.autograd.grad(demod_ref(w, sd, scale, eps), sd, gd.double())
+    d = demod_ref(w, s, scale, eps)
+    wsq = w.double()[0].pow(2).sum(dim=(2, 3))
+    mag = scale ** 2 * s.double().abs() * ((gd.double().abs() * d.pow(3)) @ wsq)
+    return gs, mag
+
+
+@pytest.mark.parametrize("b,o,i", DEMOD_CASES)
+def test_demod_coefficients_vs_float64(b, o, i):
+    """modconv.demod_coefficients (wgmma TF32 hi/lo GEMM) vs float64 rsqrt(scale^2 * sum_i Wsq s^2 + eps), per element
+    relative error <= DEMOD_RTOL (derived in tests/test_demod_precision.py, which also shows a TF32-only kernel misses it).
+    The cases reach every <NA, NS> instance of demod_wgmma_kernel.  Observed on an H100 80GB HBM3 (700 W power limit):
+    max 5.4e-6 (B=17, O=127, I=513), the split itself ~5e-7 (emulated): the tensor core's fp32 accumulation over the k-steps
+    dominates, growing with I -- so the bound stays at 8e-6 rather than 4x the observed value.
+    Style gradient (_Demod.backward) vs float64 autograd, relative to the sum of |terms| of its contraction."""
+    from gangealing_b200.op.modconv import demod_coefficients
+    w, s, scale = demod_inputs(b, o, i)
+    sg = s.to(DEV).requires_grad_(True)
+    d = demod_coefficients(w.to(DEV), sg, scale)
+    assert d.shape == (b, o) and d.dtype == torch.float32
+    err = max_rel_err(d, demod_ref(w, s, scale))
+    assert err <= DEMOD_RTOL, "max relative error %.2e > %.1e" % (err, DEMOD_RTOL)
+    gd = torch.randn(b, o, generator=torch.Generator().manual_seed(o))
+    (gs,) = torch.autograd.grad(d, sg, gd.to(DEV))
+    gs_ref, mag = _demod_style_grad_ref(w, s, scale, gd)
+    excess = ((gs.double().cpu() - gs_ref).abs() - 1e-5 * mag).max().item()
+    assert excess <= 0, "style gradient error exceeds 1e-5 of |terms| by %.3e" % excess
+
+
+def test_batched_demod_matches_the_single_layer_kernel_bitwise():
+    """style_path.all_demod (one launch for every layer, csrc/modconv.cu DemodBatch) with the 256^2 generator's 13 layer
+    shapes plus an I=32 layer that forces NA=1 for the whole batch: each layer within DEMOD_RTOL of float64 and BITWISE
+    equal to demod_coefficients of that layer alone -- the same MMAs in the same k order -- and the _DemodAll.backward
+    gradients vs float64 autograd."""
+    from gangealing_b200.op import style_path
+    from gangealing_b200.op.modconv import demod_coefficients
+    b = 8
+    layers = GEN256_DEMOD_LAYERS + [(64, 32)]
+    ws, ss, scales = [], [], []
+    for j, (o, i) in enumerate(layers):
+        w, s, scale = demod_inputs(b, o, i, seed=j)
+        ws.append(w), ss.append(s), scales.append(scale)
+    sg = [s.to(DEV).requires_grad_(True) for s in ss]
+    wd = [w.to(DEV) for w in ws]
+    dm = style_path.all_demod(wd, sg, scales)
+    gds = [torch.randn(d.shape, generator=torch.Generator().manual_seed(j)) for j, d in enumerate(dm)]
+    grads = torch.autograd.grad(dm, sg, [g.to(DEV) for g in gds])
+    for j, (w, s, scale) in enumerate(zip(ws, ss, scales)):
+        err = max_rel_err(dm[j], demod_ref(w, s, scale))
+        assert err <= DEMOD_RTOL, "layer %d: max relative error %.2e" % (j, err)
+        single = demod_coefficients(wd[j], s.to(DEV), scale)
+        assert torch.equal(dm[j], single), "layer %d differs from the single-layer launch" % j
+        gs_ref, mag = _demod_style_grad_ref(w, s, scale, gds[j])
+        excess = ((grads[j].double().cpu() - gs_ref).abs() - 1e-5 * mag).max().item()
+        assert excess <= 0, "layer %d: style gradient error exceeds 1e-5 of |terms| by %.3e" % (j, excess)

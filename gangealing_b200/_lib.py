@@ -74,6 +74,9 @@ SIGNATURES = {
     "gg_flow_compose_forward": (_I, [_P] * 7 + [_L, _I, _I, _I, _P]),
     "gg_flow_compose_backward": (_I, [_P] * 10 + [_L, _I, _I, _I, _P]),
     "gg_mipmap_warp_backward": (_I, [_P] * 7 + [_I, _L] + [_I] * 6 + [_F, _F, _I, _P]),
+    "gg_laplacian_blend_workspace": (_L, [_L, _I, _I, _I, _I, _I]),
+    "gg_laplacian_blend_forward": (_I, [_P] * 6 + [_L, _I, _I, _I, _I, _I, _P]),
+    "gg_laplacian_blend_backward": (_I, [_P] * 9 + [_L, _I, _I, _I, _I, _I, _P]),
 }
 
 _dll = None

@@ -10,6 +10,7 @@ It pre-registers, under the reference's module names, the modules that sit direc
   models.stylegan2.op (+ .upfirdn2d, .fused_act, .conv2d_gradfix)   <- gangealing_b200.op
   models.spatial_transformers.antialiased_sampling                  <- gangealing_b200.stn.sampling
   utils.splat2d_cuda (+ .functional, .splat)                        <- gangealing_b200.splat2d
+  utils.laplacian_blending (LaplacianBlender)                       <- gangealing_b200.splat2d.blend
 so the reference never reaches its import-time JIT builds (`torch.utils.cpp_extension.load`, op/upfirdn2d.py:9-16,
 op/fused_act.py:10-17, utils/splat2d_cuda/functional.py:9-27 -- the last of which no longer compiles on modern
 torch).  Everything above those modules is the reference's own code, untouched.
@@ -46,4 +47,7 @@ def install(force=False):
     splat_mod = types.ModuleType("utils.splat2d_cuda.splat")
     splat_mod.Splat2D, splat_mod.splat2d = _splat.Splat2D, _splat.splat2d
     register("utils.splat2d_cuda.splat", splat_mod)
+    blend_mod = types.ModuleType("utils.laplacian_blending")     # the reference's needs cv2 for its 1-D Gaussians
+    blend_mod.LaplacianBlender = _splat.LaplacianBlender
+    register("utils.laplacian_blending", blend_mod)
     return pkg

@@ -20,6 +20,7 @@ def cuda_ops():
         from .splat2d import nn_argmin as _nn_argmin
         from .splat2d import splat2d as _splat2d
         from .splat2d import splat2d_lookup as _splat2d_lookup
+        from .splat2d import laplacian_blend as _laplacian_blend
         from .op import feature_distance as _fd
         from .op import vgg_pool as _vp
         _cached = types.SimpleNamespace(
@@ -42,6 +43,7 @@ def cuda_ops():
             splat2d=_splat2d,
             splat2d_lookup=_splat2d_lookup,               # uncongeal_points' grid lookup fused into the splat
             nn_argmin=_nn_argmin,                         # congeal_points' brute-force search without the distance tensor
+            laplacian_blend=_laplacian_blend,             # splat_points(blend_alg='laplacian*'): fused Gaussian stacks
             feature_distance=_fd.feature_distance,
             feature_distance_stacked=_fd.feature_distance_stacked,   # both images' features from ONE backbone pass
             bias_relu_pool=_vp.bias_relu_pool,            # VGG slice boundary: bias + ReLU + 2x2 max-pool, one pass each way

@@ -1,9 +1,10 @@
 """Mirror of reference utils/splat2d_cuda/__init__.py (`from .splat import *`)."""
 import torch.nn as nn
 
+from .blend import LaplacianBlender, laplacian_blend, splat_points
 from .functional import nn_argmin, splat2d, splat2d_lookup
 
-__all__ = ["Splat2D", "splat2d", "splat2d_lookup", "nn_argmin"]
+__all__ = ["Splat2D", "splat2d", "splat2d_lookup", "nn_argmin", "laplacian_blend", "LaplacianBlender", "splat_points"]
 
 
 class Splat2D(nn.Module):

@@ -8,6 +8,7 @@ import torch
 import torch.nn as nn
 
 from ..opset import cuda_ops
+from ..splat2d.blend import BLEND_PRESETS
 from ..stylegan2.networks import ConvLayer, EqualLinear, ResBlock, channel_table
 from .heads import FlowHead, SimilarityHead
 from .sampling import BilinearDownsample
@@ -350,10 +351,14 @@ class ComposedSTN(nn.Module):
         return (pointsB, congealed_img) if return_congealed_img else pointsB
 
     def uncongeal_and_splat(self, imgB, points_congealed, colors, sigma, opacity, alpha_channel=None, output_resolution=None,
-                            iters=1, normalize_input_points=False, **stn_forward_kwargs):
-        """`uncongeal_points(imgB, points)` followed by `splat_points(imgB, points, sigma, opacity, colors=...)` (reference
-        applications/propagate_to_images.py:44-78 + utils/vis_tools/helpers.py:134-194, alpha blending) with the grid lookup
-        fused into the first splat's point load (csrc/splat.cu LOOKUP).  -> (propagated images, points (N, P, 2) in pixels)."""
+                            iters=1, normalize_input_points=False, blend_alg="alpha", **stn_forward_kwargs):
+        """`uncongeal_points(imgB, points)` followed by `splat_points(imgB, points, sigma, opacity, colors=...,
+        blend_alg=...)` (reference applications/propagate_to_images.py:44-78 + utils/vis_tools/helpers.py:134-194) with the
+        grid lookup fused into the first splat's point load (csrc/splat.cu LOOKUP).  blend_alg: 'alpha' (alpha compositing),
+        'laplacian' or 'laplacian_light' (the op set's laplacian_blend with splat_points' presets).
+        -> (propagated images, points (N, P, 2) in pixels)."""
+        if blend_alg != "alpha" and blend_alg not in BLEND_PRESETS:
+            raise ValueError("blend_alg must be 'alpha', 'laplacian' or 'laplacian_light' (got %r)" % (blend_alg,))
         assert imgB.size(0) == points_congealed.size(0)
         if normalize_input_points:
             points_congealed = SpatialTransformer.normalize(points_congealed, imgB.size(-1), self.stn_in_size)
@@ -372,6 +377,11 @@ class ComposedSTN(nn.Module):
             pointsB = SpatialTransformer.unnormalize(self.stns[0]._lookup(gridB, points_congealed), res, res)
             prop_obj = self.ops.splat2d(blank_img, pointsB, colors, sig, False)
         prop_mask = self.ops.splat2d(blank_mask, pointsB, alpha_channel, sig, True) * opacity
+        if blend_alg != "alpha":
+            kw = BLEND_PRESETS[blend_alg]
+            prop_obj, prop_mask = prop_obj.to(imgB.device), prop_mask.to(imgB.device)
+            return self.ops.laplacian_blend(imgB, prop_obj, prop_mask, kw["levels"], kw["gaussian_kernel_size"],
+                                            kw["gaussian_sigma"]), pointsB
         return prop_mask * prop_obj + (1 - prop_mask) * imgB, pointsB
 
     def congeal_points(self, imgA, pointsA, output_resolution=None, iters=1, normalize_input_points=True,

@@ -395,6 +395,24 @@ GG_API int gg_splat2d_lookup_forward(float* out, float* points_out, void* worksp
                                      int soft_normalize, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Laplacian pyramid blending, csrc/blend.cu: reference utils/laplacian_blending.py:56-107 (`LaplacianBlender.get_stacks` +
+ * `forward`), as called by splat_points(blend_alg='laplacian' | 'laplacian_light') (utils/vis_tools/helpers.py:186-193).
+ *   out = sum_{l<L-1} lerp(A_l - A_{l+1}, B_l - B_{l+1}, M_l) + lerp(A_{L-1}, B_{L-1}, M_{L-1}),
+ *   G_0 = x, G_{l+1} = T_l G_l: a replicate-padded Gaussian blur with the 1-D taps of row l (applied along x, then y).
+ * img0 / img1 / out / grads: (N, C, H, W) fp32 NCHW; mask / grad_mask: (N, 1, H, W) fp32 (broadcast over channels);
+ * taps: DEVICE fp32 (levels-1, width), each row the normalised 1-D Gaussian of its level (NULL when levels == 1);
+ * width odd, 1 <= width <= 63 (GG_ERR_BAD_ARG for even / non-positive, GG_ERR_UNSUPPORTED above 63); levels >= 1.
+ * `workspace`: gg_laplacian_blend_workspace(N, C, H, W, levels, backward) bytes (0 when levels == 1, NULL allowed then).
+ * Backward returns all three gradients (gather form, no atomics; bitwise reproducible).  Neither call synchronises. */
+GG_API int64_t gg_laplacian_blend_workspace(int64_t N, int C, int H, int W, int levels, int backward);
+GG_API int gg_laplacian_blend_forward(float* out, void* workspace, const float* img0, const float* img1, const float* mask,
+                                      const float* taps, int64_t N, int C, int H, int W, int levels, int width, void* stream);
+GG_API int gg_laplacian_blend_backward(float* grad_img0, float* grad_img1, float* grad_mask, void* workspace,
+                                       const float* grad_out, const float* img0, const float* img1, const float* mask,
+                                       const float* taps, int64_t N, int C, int H, int W, int levels, int width,
+                                       void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Training-loop bookkeeping (SURVEY.md 8(f) rank 3), csrc/optim.cu.
  *   gg_adam_ema_step: reference train.py:126-134 -- torch.optim.Adam.step() for every parameter of both optimisers and the
  *     EMA `accumulate(t_ema, t_module)` (models/__init__.py:19-24) -- as one multi-tensor pass.

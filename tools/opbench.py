@@ -281,9 +281,68 @@ def stn_rows(B, dev, timeit, peak, json_path):
                    "rows": rows}, open(json_path, "w"), indent=1)
 
 
+FP32_PEAK_TFLOPS = 67.0   # H100 SXM data sheet, dense FP32 (700 W)
+
+
+def blend_rows(dev, timeit, peak, json_path):
+    """Laplacian pyramid blending (splat_points(blend_alg='laplacian*')): the reference's formulation (2-D depthwise
+    convolution per level, materialised stacks; oracle.blend.laplacian_blend_conv2d_ref on the GPU) vs the fused op,
+    forward and forward+backward.  Bounds per call: FMA = 2 (2C+1) (L-1) width per pixel (separable blur, both passes),
+    bytes = 4 N H W (3C+1) (read img0, img1, mask, write out); each as a share of the data-sheet peak."""
+    from oracle import blend as OB
+    from gangealing_b200.splat2d import laplacian_blend
+    props = torch.cuda.get_device_properties(0)
+    try:
+        import subprocess
+        power = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
+                               capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
+    except Exception as e:   # noqa: BLE001 -- report, do not fail the measurement
+        power = "unknown (%s)" % e
+    print("card: %s | power limit, max SM clock: %s" % (props.name, power))
+    presets = {"laplacian": (5, 45, 1.0), "laplacian_light": (3, 11, 0.5)}
+    rows = []
+    g = torch.Generator(device=dev).manual_seed(0)
+    for n, res in [(4, 1024), (8, 512)]:
+        c = 3
+        img0 = torch.rand(n, c, res, res, device=dev, generator=g) * 2 - 1
+        img1 = torch.rand(n, c, res, res, device=dev, generator=g) * 2 - 1
+        mask = torch.rand(n, 1, res, res, device=dev, generator=g)
+        gout = torch.rand(n, c, res, res, device=dev, generator=g)
+        for name, (levels, k, s) in presets.items():
+            fma = 2 * (2 * c + 1) * (levels - 1) * k * n * res * res
+            nbytes = 4 * n * res * res * (3 * c + 1)
+            t_fma, t_mem = fma / (FP32_PEAK_TFLOPS * 0.5e12) * 1e3, nbytes / (peak * 1e6)   # ms at peak (1 FMA = 2 FLOP)
+            ms_ref = timeit(lambda i: OB.laplacian_blend_conv2d_ref(img0, img1, mask, levels, k, s), 1, iters=5, warmup=2)
+            ms_fwd = timeit(lambda i: laplacian_blend(img0, img1, mask, levels, k, s), 1, iters=20, warmup=3)
+            leaves = [t.clone().requires_grad_(True) for t in (img0, img1, mask)]
+
+            def fwd_bwd(i):
+                out = laplacian_blend(*leaves, levels, k, s)
+                return torch.autograd.grad(out, leaves, gout)
+            ms_fb = timeit(fwd_bwd, 1, iters=10, warmup=3)
+            err = (laplacian_blend(img0, img1, mask, levels, k, s)
+                   - OB.laplacian_blend_conv2d_ref(img0, img1, mask, levels, k, s)).abs().max().item()
+            bound = "FMA" if t_fma >= t_mem else "HBM"
+            row = {"preset": name, "N": n, "res": res, "reference_ms": ms_ref, "fused_fwd_ms": ms_fwd,
+                   "fused_fwd_bwd_ms": ms_fb, "fma_G": fma / 1e9, "MB": nbytes / 1e6,
+                   "fwd_fma_frac_of_peak": t_fma / ms_fwd, "fwd_bytes_frac_of_peak": t_mem / ms_fwd, "binding": bound,
+                   "speedup_vs_reference": ms_ref / ms_fwd, "max_abs_diff_vs_reference": err}
+            rows.append(row)
+            print("%-16s N=%d %4d^2  ref %8.3f ms | fused fwd %7.3f ms  fwd+bwd %7.3f ms | x%5.1f vs ref | fwd: FMA %.1f G "
+                  "= %4.1f%% of FP32 peak, bytes %.0f MB = %4.1f%% of HBM peak -> %s-bound | max|diff| %.2e" % (
+                      name, n, res, ms_ref, ms_fwd, ms_fb, ms_ref / ms_fwd, fma / 1e9, 100 * t_fma / ms_fwd, nbytes / 1e6,
+                      100 * t_mem / ms_fwd, bound, err))
+    if json_path:
+        os.makedirs(os.path.dirname(os.path.abspath(json_path)), exist_ok=True)
+        json.dump({"card": props.name, "power_limit_and_max_sm_clock": power, "fp32_peak_tflops": FP32_PEAK_TFLOPS,
+                   "peak_gbs": peak, "what": "Laplacian blending: reference 2-D conv formulation vs fused op (CUDA events)",
+                   "rows": rows}, open(json_path, "w"), indent=1)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--stn", action="store_true", help="the STN sampling path: reference / two-pass / one-pass")
+    ap.add_argument("--blend", action="store_true", help="Laplacian blending: reference formulation vs the fused op")
     ap.add_argument("--ref", action="store_true", help="time the reference's own CUDA kernels (oracle/_ref) next to ours")
     ap.add_argument("--graph", action="store_true", help="time CUDA-graph replays (device time without launch overhead)")
     ap.add_argument("--batch", type=int, default=5)
@@ -312,6 +371,9 @@ def main():
 
     if args.stn:
         stn_rows(B, dev, timeit, peak, args.json)
+        return
+    if args.blend:
+        blend_rows(dev, timeit, peak, args.json)
         return
     if args.ref:
         reference_bar(B, dev, k4, timeit, pool_count, peak, args.json)

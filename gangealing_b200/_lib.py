@@ -77,6 +77,9 @@ SIGNATURES = {
     "gg_laplacian_blend_workspace": (_L, [_L, _I, _I, _I, _I, _I]),
     "gg_laplacian_blend_forward": (_I, [_P] * 6 + [_L, _I, _I, _I, _I, _I, _P]),
     "gg_laplacian_blend_backward": (_I, [_P] * 9 + [_L, _I, _I, _I, _I, _I, _P]),
+    "gg_tv_per_sample": (_I, [_P, _P, _L, _I, _I, _P]),
+    "gg_pck_transfer_workspace": (_L, [_L, _L, _I]),
+    "gg_pck_transfer": (_I, [_P] * 14 + [_L, _L, _I, _I, _I, _I, _I, _P]),
 }
 
 _dll = None

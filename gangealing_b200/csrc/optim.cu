@@ -14,6 +14,7 @@
 //                      forward and ~25 backward on a 4 MB tensor; here one reduction kernel forward (+ finish) and one
 //                      gather-form (atomic-free, deterministic) kernel backward.
 #include "common.cuh"
+#include "tv.cuh"
 
 namespace gg {
 namespace {
@@ -144,14 +145,6 @@ scale_cast_multi_kernel(const ScaleTensor* __restrict__ table, const int* __rest
 }
 
 // ------------------------------------------------------------------------------------------------ total variation
-__device__ __forceinline__ float huber(float d) {            // loss.py:7: where(a <= 1, 0.5 a^2, a - 0.5), a = |d|
-  const float a = fabsf(d);
-  return a <= 1.f ? 0.5f * a * a : a - 0.5f;
-}
-__device__ __forceinline__ float huber_grad(float d) {       // d/dd
-  return fabsf(d) <= 1.f ? d : (d > 0.f ? 1.f : -1.f);
-}
-
 constexpr int kTvThreads = 256;
 
 // partial[block] = sum over the block's elements of huber(dy)*inv_y + huber(dx)*inv_x

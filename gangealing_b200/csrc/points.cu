@@ -11,6 +11,7 @@
 // index -- exactly argmin's rule.  The distance is evaluated with the reference's expanded expression and operation order
 // (separately rounded products, no FMA contraction), so near-ties resolve like the reference's.
 #include "common.cuh"
+#include "points.cuh"
 
 namespace gg {
 namespace {
@@ -76,6 +77,26 @@ __global__ void nn_unpack_kernel(int64_t* __restrict__ index, const unsigned lon
 }
 
 }  // namespace
+
+int nn_argmin_search(unsigned long long* best, const float* grid, const float* points, int64_t N, int64_t P, int HW,
+                     cudaStream_t st) {
+  const int64_t total = N * P;
+  nn_init_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(best, total);
+  GG_CHECK_LAUNCH("nn_init launch");
+  const int64_t pblocks = (P + kNNThreads - 1) / kNNThreads;
+  if (pblocks > 0x7fffffffLL) return fail(GG_ERR_BAD_ARG, "nn_argmin: too many points");
+  // split the grid entries over CTAs until the machine is filled ~2x (each split scans >= one tile)
+  int splits = static_cast<int>((2LL * sm_count() + pblocks * N - 1) / (pblocks * N));
+  const int max_splits = (HW + kNNTile - 1) / kNNTile;
+  if (splits > max_splits) splits = max_splits;
+  if (splits < 1) splits = 1;
+  if (splits > 65535) splits = 65535;
+  nn_argmin_kernel<<<dim3(static_cast<unsigned>(pblocks), static_cast<unsigned>(splits), static_cast<unsigned>(N)), kNNThreads, 0, st>>>(
+      best, grid, points, P, HW, splits);
+  GG_CHECK_LAUNCH("nn_argmin launch");
+  return GG_OK;
+}
+
 }  // namespace gg
 
 using namespace gg;
@@ -94,19 +115,8 @@ int gg_nn_argmin(int64_t* index, void* workspace, const float* grid, const float
   auto st = static_cast<cudaStream_t>(stream);
   auto* best = static_cast<unsigned long long*>(workspace);
   const int64_t total = N * P;
-  nn_init_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(best, total);
-  GG_CHECK_LAUNCH("nn_init launch");
-  const int64_t pblocks = (P + kNNThreads - 1) / kNNThreads;
-  if (pblocks > 0x7fffffffLL) return fail(GG_ERR_BAD_ARG, "nn_argmin: too many points");
-  // split the grid entries over CTAs until the machine is filled ~2x (each split scans >= one tile)
-  int splits = static_cast<int>((2LL * sm_count() + pblocks * N - 1) / (pblocks * N));
-  const int max_splits = (HW + kNNTile - 1) / kNNTile;
-  if (splits > max_splits) splits = max_splits;
-  if (splits < 1) splits = 1;
-  if (splits > 65535) splits = 65535;
-  nn_argmin_kernel<<<dim3(static_cast<unsigned>(pblocks), static_cast<unsigned>(splits), static_cast<unsigned>(N)), kNNThreads, 0, st>>>(
-      best, grid, points, P, HW, splits);
-  GG_CHECK_LAUNCH("nn_argmin launch");
+  const int rc = nn_argmin_search(best, grid, points, N, P, HW, st);
+  if (rc != GG_OK) return rc;
   nn_unpack_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(index, best, total);
   GG_CHECK_LAUNCH("nn_unpack launch");
   return GG_OK;

@@ -23,6 +23,7 @@ def cuda_ops():
         from .splat2d import laplacian_blend as _laplacian_blend
         from .op import feature_distance as _fd
         from .op import vgg_pool as _vp
+        from .evaluation import ops as _ev
         _cached = types.SimpleNamespace(
             name="sm_90a",
             upfirdn2d=_op.upfirdn2d,
@@ -48,5 +49,7 @@ def cuda_ops():
             feature_distance_stacked=_fd.feature_distance_stacked,   # both images' features from ONE backbone pass
             bias_relu_pool=_vp.bias_relu_pool,            # VGG slice boundary: bias + ReLU + 2x2 max-pool, one pass each way
             bias_relu_pool_supported=_vp.supported,
+            tv_per_sample=_ev.tv_per_sample,              # match_flows / flow_scores: per-sample smoothness, one launch
+            pck_transfer_points=_ev.pck_transfer_points,  # PCK-Transfer: congeal + search + lookup + score, one call
         )
     return _cached

@@ -78,6 +78,32 @@ def unravel_index(indices, shape):
     return torch.stack(coord, dim=-1)
 
 
+def match_pick(tv):
+    """match_flows' choice (reference spatial_transformer.py:269-278) from the per-sample smoothness of the 4N batch
+    [A, B, flip(A), flip(B)]: 0 = neither flipped, 1 = A flipped, 2 = B flipped, 3 = both.  -> (N, 1, 1, 1) int64."""
+    tvA, tvB, tvAf, tvBf = tv.chunk(4, dim=0)
+    return torch.stack([tvA + tvB, tvAf + tvB, tvA + tvBf, tvAf + tvBf], 0).argmin(dim=0).view(tvA.size(0), 1, 1, 1)
+
+
+def flip_key_points(pick, pointsA, pointsB, permutation, size):
+    """match_flows' key-point update (reference spatial_transformer.py:282-292) for images of width `size`: mirror x where
+    an image was flipped and relabel with `permutation`.  The reference's quirk is kept: when pointsB is given, the second
+    relabelling permutes pointsA again (where B was flipped) and never touches pointsB.  -> (pointsA, pointsB or None)."""
+    keepA = (pick % 2 == 0).view(pick.size(0), 1)
+    pointsA = pointsA.clone()
+    pointsA[:, :, 0] = torch.where(keepA, pointsA[:, :, 0], size - 1 - pointsA[:, :, 0])
+    if permutation is not None:
+        pointsA = torch.where(keepA.view(pick.size(0), 1, 1), pointsA, pointsA[:, permutation])
+    if pointsB is None:
+        return pointsA, None
+    keepB = (pick <= 1).view(pick.size(0), 1)
+    pointsB = pointsB.clone()
+    pointsB[:, :, 0] = torch.where(keepB, pointsB[:, :, 0], size - 1 - pointsB[:, :, 0])
+    if permutation is not None:
+        pointsA = torch.where(keepB.view(pick.size(0), 1, 1), pointsA, pointsA[:, permutation])
+    return pointsA, pointsB
+
+
 def _pack(values, flags):
     out = [values[0]] + [v for v, f in zip(values[1:], flags) if f]
     return out[0] if len(out) == 1 else out
@@ -425,6 +451,36 @@ class ComposedSTN(nn.Module):
         if return_flip_indices:
             out.append(use_flip)
         return out[0] if len(out) == 1 else out
+
+    def match_flows(self, imgA, imgB, pointsA, pointsB=None, permutation=None, **stn_forward_kwargs):
+        """Flip neither, one or both images of each pair so that their residual flows are smoothest; update the key points
+        to follow (reference :242-295, quirks in flip_key_points).  ONE STN forward over [A, B, flip(A), flip(B)] and one
+        per-sample smoothness (the op set's tv_per_sample).
+        -> (imgA, imgB, pointsA, [pointsB,] pick) with pick (N, 1, 1, 1) in {0: none, 1: A, 2: B, 3: both flipped}."""
+        imgA_flip, imgB_flip = imgA.flip(3,), imgB.flip(3,)
+        _, flows = self.forward(torch.cat([imgA, imgB, imgA_flip, imgB_flip], 0), return_flow=True, **stn_forward_kwargs)
+        pick = match_pick(self.ops.tv_per_sample(flows))
+        imgA = torch.where(pick % 2 == 0, imgA, imgA_flip)
+        imgB = torch.where(pick <= 1, imgB, imgB_flip)
+        pointsA, pointsB_out = flip_key_points(pick, pointsA, pointsB, permutation, imgA.size(-1))
+        if pointsB is not None:
+            return imgA, imgB, pointsA, pointsB_out, pick
+        return imgA, imgB, pointsA, pick
+
+    def _matrix_flow_grid(self, input_img, iters=1, **stn_forward_kwargs):
+        """forward(input_img) of a similarity -> flow STN, returning what point transfer reads from it: the similarity
+        matrix (N, 2, 3), the residual flow (N, F, F, 2) and the composed sampling grid (N, F, F, 2).  The calls are
+        forward's (same arguments, same order), so each output equals the one congeal_points / uncongeal_points get."""
+        if self.transforms != ["similarity", "flow"] or self.num_heads > 1:
+            raise ValueError("point transfer from one forward needs a single-head similarity -> flow ComposedSTN")
+        sim, flow = self.stns
+        out, _, matrix = sim(input_img, return_warp=True, return_flow=True, return_intermediates=False,
+                             input_img_for_sampling=input_img, base_warp=None, output_resolution=self.stn_in_size,
+                             unfold=False, iters=iters, alpha=None, warp_policy="cartesian", **stn_forward_kwargs)
+        _, grid, delta = flow(out, return_warp=True, return_flow=True, return_intermediates=False,
+                              input_img_for_sampling=input_img, base_warp=matrix, output_resolution=None, unfold=False,
+                              iters=1, alpha=None, warp_policy="cartesian", **stn_forward_kwargs)
+        return matrix, delta, grid
 
     def load_single_state_dict(self, state_dict, index, strict=True):
         return self.stns[index].load_state_dict(state_dict, strict)

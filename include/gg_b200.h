@@ -395,6 +395,33 @@ GG_API int gg_splat2d_lookup_forward(float* out, float* points_out, void* worksp
                                      int soft_normalize, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * PCK-Transfer evaluation, csrc/pck.cu.
+ *   gg_tv_per_sample: reference models/losses/loss.py:4-12 total_variation_loss(flow, reduce_batch=False) for a (N, H, W, 2)
+ *     fp32 flow: out[n] = mean huber|d/dx| + mean huber|d/dy| of sample n.  One CTA per sample, no atomics (bitwise
+ *     reproducible); H, W >= 2.
+ *   gg_pck_transfer: one transfer direction of applications/pck.py:145-166 for B source -> destination pairs, i.e.
+ *     ComposedSTN.transfer_points (spatial_transformer.py:159-198, :631-672, :141-157) + the PCK test, on quantities of ONE
+ *     STN forward (replaces torch.inverse, the (N, H, W, P) distance tensor, argmin, unravel_index, grid_sample and ~40
+ *     elementwise launches per direction):
+ *       points / gt_points (B, P, 2) pixels of the S x S source / destination image; visible (B, P) 0/1 or NULL (all);
+ *       thresh (B,) per-destination threshold; alphas (A,) DEVICE, 1 <= A <= 8;
+ *       matrix_src (B, 2, 3) the source's similarity matrix (first STN);
+ *       composed STN: delta_src (B, F, F, 2) the source's residual flow, identity (F, F, 2) the identity flow, grid_dst
+ *       (B, grid_h, grid_w, 2) the destination's composed sampling grid, grid_h == grid_w == F; matrix_dst unused;
+ *       similarity-only STN: delta_src = identity = grid_dst = NULL, matrix_dst (B, 2, 3) the destination's matrix.
+ *     counts (A,) int64 is ACCUMULATED: counts[a] += #{(b, p): visible and |est - gt| <= alphas[a] * thresh[b]} (integer
+ *     atomics: deterministic).  est_points (B, P, 2) and nn_index (B, P) (flat F x F index, composed STN) may be NULL.
+ *     `workspace`: gg_pck_transfer_workspace(B, P, F) bytes (F = 0 for a similarity-only STN).  No sync, no allocation.
+ * ---------------------------------------------------------------------------------------------- */
+GG_API int gg_tv_per_sample(float* out, const float* flow, int64_t N, int H, int W, void* stream);
+GG_API int64_t gg_pck_transfer_workspace(int64_t B, int64_t P, int F);
+GG_API int gg_pck_transfer(int64_t* counts, float* est_points, int64_t* nn_index, void* workspace, const float* points,
+                           const float* gt_points, const float* visible, const float* thresh, const float* alphas,
+                           const float* matrix_src, const float* matrix_dst, const float* delta_src, const float* identity,
+                           const float* grid_dst, int64_t B, int64_t P, int A, int S, int F, int grid_h, int grid_w,
+                           void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Laplacian pyramid blending, csrc/blend.cu: reference utils/laplacian_blending.py:56-107 (`LaplacianBlender.get_stacks` +
  * `forward`), as called by splat_points(blend_alg='laplacian' | 'laplacian_light') (utils/vis_tools/helpers.py:186-193).
  *   out = sum_{l<L-1} lerp(A_l - A_{l+1}, B_l - B_{l+1}, M_l) + lerp(A_{L-1}, B_{L-1}, M_{L-1}),

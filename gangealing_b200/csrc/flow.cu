@@ -6,7 +6,7 @@
 //                               identity_flow.lerp(flow, alpha)
 // One thread per full-resolution flow pixel; tensors are KB-sized, so the cost is launch latency and the
 // win is launch count.  Algorithmic bytes per sample (K=1, 16x16 -> 128x128): mask 0.59 MB + outputs 0.26 MB.
-#include "common.cuh"
+#include "flow_compose.cuh"
 
 namespace gg {
 namespace {
@@ -39,51 +39,21 @@ flow_compose_fwd_kernel(float* __restrict__ delta_out, float* __restrict__ flow_
        idx += static_cast<int64_t>(gridDim.x) * blockDim.x) {
     int64_t n; int sy, sx, h, w;
     decode(p, idx, n, sy, sx, h, w);
-    // softmax over the 9 logits
-    float lg[9], mx = -INFINITY;
-#pragma unroll
-    for (int k = 0; k < 9; ++k) { lg[k] = mask[mask_index(p, n, k, sy, sx, h, w)]; mx = fmaxf(mx, lg[k]); }
-    float sum = 0.f;
-#pragma unroll
-    for (int k = 0; k < 9; ++k) { lg[k] = expf(lg[k] - mx); sum += lg[k]; }
-    const float inv = 1.f / sum;
-    // convex combination of the 3x3 neighbourhood of s*flow (zero padded, F.unfold padding=1)
-    float dx = 0.f, dy = 0.f;
-#pragma unroll
-    for (int k = 0; k < 9; ++k) {
-      const int hh = h + k / 3 - 1, ww = w + k % 3 - 1;
-      if (hh >= 0 && hh < p.h && ww >= 0 && ww < p.w) {
-        const float2 f = *reinterpret_cast<const float2*>(low + ((n * p.h + hh) * static_cast<int64_t>(p.w) + ww) * 2);
-        const float pk = lg[k] * inv;
-        dx = fmaf(pk, static_cast<float>(p.s) * f.x, dx);
-        dy = fmaf(pk, static_cast<float>(p.s) * f.y, dy);
-      }
-    }
+    float pk[9], fx[9], fy[9];
+    const float2 u = convex_upsample(low, mask, n, p.h, p.w, p.s, sy, sx, h, w, pk, fx, fy);
     const int Y = h * p.s + sy, X = w * p.s + sx;
     const int64_t pix = (static_cast<int64_t>(Y) * (p.w * p.s) + X) * 2;
     const int64_t o = n * (p.h * p.s) * static_cast<int64_t>(p.w * p.s) * 2 + pix;
-    *reinterpret_cast<float2*>(delta_out + o) = make_float2(dx, dy);
+    *reinterpret_cast<float2*>(delta_out + o) = u;
     if (flow_out) {
       const float2 id = *reinterpret_cast<const float2*>(identity + pix);
-      float gx = id.x + dx, gy = id.y + dy;
-      if (base) {  // [gx, gy, 1] @ M^T   (warping_heads.py:268-277)
-        const float* M = base + n * 6;
-        const float tx = M[0] * gx + M[1] * gy + M[2];
-        const float ty = M[3] * gx + M[4] * gy + M[5];
-        gx = tx; gy = ty;
-      }
-      if (alpha) {  // identity.lerp(flow, alpha) = identity + alpha*(flow - identity)
-        const float a = alpha[n];
-        gx = id.x + a * (gx - id.x);
-        gy = id.y + a * (gy - id.y);
-      }
-      *reinterpret_cast<float2*>(flow_out + o) = make_float2(gx, gy);
+      *reinterpret_cast<float2*>(flow_out + o) = compose_flow(id, u.x, u.y, base, alpha, n);
     }
   }
 }
 
-// backward of one full-resolution pixel: softmax weights pk, the scaled neighbourhood (fx, fy), the gradient arriving at
-// delta (gdx, gdy) and, with g_flow and base, this pixel's terms of d loss / d base (v, zero otherwise)
+// backward of one full-resolution pixel: the forward's convex up-sampling (softmax weights, scaled neighbourhood), the
+// gradient arriving at delta (gdx, gdy) and, with g_flow and base, this pixel's terms of d loss / d base (v, zero otherwise)
 struct PixelGrad {
   float pk[9], fx[9], fy[9];
   float gdx, gdy;
@@ -98,26 +68,7 @@ __device__ __forceinline__ void pixel_grad(const FlowParams& p, int64_t n, int s
   const int Y = h * p.s + sy, X = w * p.s + sx;
   const int64_t pix = (static_cast<int64_t>(Y) * (p.w * p.s) + X) * 2;
   const int64_t o = n * (p.h * p.s) * static_cast<int64_t>(p.w * p.s) * 2 + pix;
-  // recompute softmax and the neighbourhood
-  float mx = -INFINITY;
-#pragma unroll
-  for (int k = 0; k < 9; ++k) { r.pk[k] = mask[mask_index(p, n, k, sy, sx, h, w)]; mx = fmaxf(mx, r.pk[k]); }
-  float sum = 0.f;
-#pragma unroll
-  for (int k = 0; k < 9; ++k) { r.pk[k] = expf(r.pk[k] - mx); sum += r.pk[k]; }
-  const float inv = 1.f / sum;
-  float dx = 0.f, dy = 0.f;
-#pragma unroll
-  for (int k = 0; k < 9; ++k) {
-    r.pk[k] *= inv;
-    const int hh = h + k / 3 - 1, ww = w + k % 3 - 1;
-    r.fx[k] = 0.f; r.fy[k] = 0.f;
-    if (hh >= 0 && hh < p.h && ww >= 0 && ww < p.w) {
-      const float2 f = *reinterpret_cast<const float2*>(low + ((n * p.h + hh) * static_cast<int64_t>(p.w) + ww) * 2);
-      r.fx[k] = static_cast<float>(p.s) * f.x; r.fy[k] = static_cast<float>(p.s) * f.y;
-    }
-    dx = fmaf(r.pk[k], r.fx[k], dx); dy = fmaf(r.pk[k], r.fy[k], dy);
-  }
+  const float2 d = convex_upsample(low, mask, n, p.h, p.w, p.s, sy, sx, h, w, r.pk, r.fx, r.fy);
 #pragma unroll
   for (int q = 0; q < 6; ++q) r.v[q] = 0.f;
   // gradient arriving at delta
@@ -128,7 +79,7 @@ __device__ __forceinline__ void pixel_grad(const FlowParams& p, int64_t n, int s
     if (alpha) { const float a = alpha[n]; gf.x *= a; gf.y *= a; }
     if (base) {
       const float2 id = *reinterpret_cast<const float2*>(identity + pix);
-      const float gx = id.x + dx, gy = id.y + dy;
+      const float gx = id.x + d.x, gy = id.y + d.y;
       const float* M = base + n * 6;
       r.v[0] = gf.x * gx; r.v[1] = gf.x * gy; r.v[2] = gf.x;
       r.v[3] = gf.y * gx; r.v[4] = gf.y * gy; r.v[5] = gf.y;
@@ -224,12 +175,6 @@ flow_base_bwd_kernel(float* __restrict__ g_base, const float* __restrict__ g_del
   }
 }
 
-inline int flow_grid(int64_t total) {
-  int64_t g = (total + 255) / 256;
-  const int64_t cap = static_cast<int64_t>(sm_count()) * 16;
-  return static_cast<int>(g < cap ? (g > 0 ? g : 1) : cap);
-}
-
 }  // namespace
 }  // namespace gg
 
@@ -246,7 +191,7 @@ int gg_flow_compose_forward(float* delta_flow, float* flow, const float* low_flo
   if (flow && !identity_flow) return fail(GG_ERR_BAD_ARG, "flow_compose_forward: flow output needs identity_flow");
   FlowParams p{N, H, W, S};
   const int64_t total = N * S * S * H * static_cast<int64_t>(W);
-  flow_compose_fwd_kernel<<<flow_grid(total), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+  flow_compose_fwd_kernel<<<grid_for(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       delta_flow, flow, low_flow, mask, identity_flow, base_warp, alpha, p, total);
   GG_CHECK_LAUNCH("flow_compose_fwd launch");
   return GG_OK;
@@ -264,11 +209,11 @@ int gg_flow_compose_backward(float* grad_mask, float* grad_low_flow, float* grad
   const int64_t total = N * S * S * H * static_cast<int64_t>(W);
   auto st = static_cast<cudaStream_t>(stream);
   if (grad_mask)
-    flow_compose_bwd_kernel<<<flow_grid(total), 256, 0, st>>>(grad_mask, grad_delta, grad_flow, low_flow, mask, identity_flow,
+    flow_compose_bwd_kernel<<<grid_for(total, 256), 256, 0, st>>>(grad_mask, grad_delta, grad_flow, low_flow, mask, identity_flow,
                                                              base_warp, alpha, p, total);
   if (grad_low_flow) {
     const int64_t entries = N * H * static_cast<int64_t>(W);
-    flow_low_bwd_kernel<<<flow_grid(entries * 32), 256, 0, st>>>(grad_low_flow, grad_delta, grad_flow, low_flow, mask,
+    flow_low_bwd_kernel<<<grid_for(entries * 32, 256), 256, 0, st>>>(grad_low_flow, grad_delta, grad_flow, low_flow, mask,
                                                                  identity_flow, base_warp, alpha, p, entries);
   }
   if (grad_base_warp && grad_flow && base_warp) {

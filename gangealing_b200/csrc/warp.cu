@@ -13,7 +13,7 @@
 //
 // HBM-bound in principle (algorithmic bytes 4*N*(C*Hs*Ws + C*Ho*Wo + 2*Ho*Wo)) but at GANgealing's sizes
 // (3 x 128^2 .. 3 x 512^2 per sample) the whole working set is L2-resident and the win is launch count.
-#include "common.cuh"
+#include "flow_compose.cuh"
 
 namespace gg {
 namespace {
@@ -63,8 +63,15 @@ __device__ __forceinline__ int reflect_idx(int j, int size) {  // ReflectionPad 
   return j;
 }
 
-// level i (from level i-1): ReflectionPad2d(1) + [1,3,3,1]^2/64 stride 2  (antialiased_sampling.py:111-117)
-// SRC_LEVEL: the input is the source image seen through the virtual pow2 reflect padding.
+// level i (from level i-1): ReflectionPad2d(1) + [1,3,3,1]^2/64 stride 2  (antialiased_sampling.py:111-117).
+// Row (or column) of level i-1 that the tap at j = 2*o + a - 1 (a = 0..3) of level-i row o reads; on level 1 (src_level)
+// the input is the source image (src_size) seen through the virtual pow2 reflect padding lp.
+__device__ __forceinline__ int down_tap(int j, int in_size, bool src_level, int lp, int src_size) {
+  j = reflect_idx(j, in_size);
+  if (src_level) j = reflect_idx(j - lp, src_size);
+  return j;
+}
+
 template <typename T, bool SRC_LEVEL>
 __global__ void mip_down_kernel(float* __restrict__ out, const T* __restrict__ in, int in_h, int in_w,
                                 int src_h, int src_w, int lp, int64_t total) {
@@ -79,12 +86,10 @@ __global__ void mip_down_kernel(float* __restrict__ out, const T* __restrict__ i
     float acc = 0.f;
 #pragma unroll
     for (int a = 0; a < 4; ++a) {
-      int yy = reflect_idx(2 * y + a - 1, in_h);
-      if (SRC_LEVEL) yy = reflect_idx(yy - lp, src_h);
+      const int yy = down_tap(2 * y + a - 1, in_h, SRC_LEVEL, lp, src_h);
 #pragma unroll
       for (int b = 0; b < 4; ++b) {
-        int xx = reflect_idx(2 * x + b - 1, in_w);
-        if (SRC_LEVEL) xx = reflect_idx(xx - lp, src_w);
+        const int xx = down_tap(2 * x + b - 1, in_w, SRC_LEVEL, lp, src_w);
         const int64_t pos = SRC_LEVEL ? (plane * src_h + yy) * static_cast<int64_t>(src_w) + xx
                                       : (plane * in_h + yy) * static_cast<int64_t>(in_w) + xx;
         acc = fmaf(Cvt<T>::to_f(in[pos]), f[a] * f[b] * (1.f / 64.f), acc);
@@ -110,12 +115,10 @@ __global__ void mip_down_bwd_kernel(float* __restrict__ grad_in, const float* __
     const float f[4] = {1.f, 3.f, 3.f, 1.f};
 #pragma unroll
     for (int a = 0; a < 4; ++a) {
-      int yy = reflect_idx(2 * y + a - 1, in_h);
-      if (SRC_LEVEL) yy = reflect_idx(yy - lp, src_h);
+      const int yy = down_tap(2 * y + a - 1, in_h, SRC_LEVEL, lp, src_h);
 #pragma unroll
       for (int b = 0; b < 4; ++b) {
-        int xx = reflect_idx(2 * x + b - 1, in_w);
-        if (SRC_LEVEL) xx = reflect_idx(xx - lp, src_w);
+        const int xx = down_tap(2 * x + b - 1, in_w, SRC_LEVEL, lp, src_w);
         const int64_t pos = SRC_LEVEL ? (plane * src_h + yy) * static_cast<int64_t>(src_w) + xx
                                       : (plane * in_h + yy) * static_cast<int64_t>(in_w) + xx;
         atomicAdd(grad_in + pos, g * (f[a] * f[b] * (1.f / 64.f)));
@@ -300,42 +303,6 @@ __device__ __forceinline__ float sample_level(const T* __restrict__ src_plane, c
   return v[0][0] * (s.wx0 * s.wy0) + v[0][1] * (s.wx1 * s.wy0) + v[1][0] * (s.wx0 * s.wy1) + v[1][1] * (s.wx1 * s.wy1);
 }
 
-template <typename T, bool MIP>
-__global__ void __launch_bounds__(256)
-warp_fwd_kernel(T* __restrict__ out, float* __restrict__ levels_out, const T* __restrict__ src,
-                const float* __restrict__ pyr, const float* __restrict__ grid, const __grid_constant__ WarpParams p,
-                int64_t total) {
-  for (int64_t idx = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; idx < total;
-       idx += static_cast<int64_t>(gridDim.x) * blockDim.x) {
-    const int ox = static_cast<int>(idx % p.wo);
-    const int64_t t = idx / p.wo;
-    const int oy = static_cast<int>(t % p.ho);
-    const int64_t n = t / p.ho;
-    const float* grid_n = grid + n * p.ho * static_cast<int64_t>(p.wo) * 2;
-    const float2 g = *reinterpret_cast<const float2*>(grid_n + (static_cast<int64_t>(oy) * p.wo + ox) * 2);
-    const SampleGeom s = sample_geom(g.x, g.y, p.hs, p.ws, p.pad_mode);
-    int l0 = 0, l1 = 0;
-    float w = 0.f;
-    if (MIP) {
-      auto grid_at = [&](int y, int x) { return *reinterpret_cast<const float2*>(grid_n + (static_cast<int64_t>(y) * p.wo + x) * 2); };
-      const LevelInfo li = level_of_detail(grid_at, oy, ox, p.ho, p.wo, p.hs, p.ws, p.max_level, p.min_level);
-      l0 = li.l0; l1 = li.l1; w = li.w;
-      if (levels_out) levels_out[idx] = li.level;
-    }
-    for (int c = 0; c < p.c; ++c) {
-      const int64_t plane = n * p.c + c;
-      const T* src_plane = src + plane * p.hs * static_cast<int64_t>(p.ws);
-      const float o0 = sample_level<T, false>(src_plane, pyr, p, plane, l0, s, nullptr, nullptr);
-      float o = o0;
-      if (MIP && l1 != l0) {
-        const float o1 = sample_level<T, false>(src_plane, pyr, p, plane, l1, s, nullptr, nullptr);
-        o = o0 + w * (o1 - o0);
-      }
-      out[(plane * p.ho + oy) * static_cast<int64_t>(p.wo) + ox] = Cvt<T>::from_f(o);
-    }
-  }
-}
-
 // ---------------------------------------------------------------- integer work of the sampler, exported for exact tests
 // One int4 per output pixel: (x0, y0) = the north-west bilinear corner in source pixels after the padding-mode transform
 // (ATen grid_sampler's floor(ix), floor(iy)), and (l0, l1) = floor / ceil of the level of detail -- produced by the SAME
@@ -358,80 +325,53 @@ sample_indices_kernel(int4* __restrict__ out, const float* __restrict__ grid, co
   }
 }
 
-// ---------------------------------------------------------------- the STN's sampling in ONE pass
-// north_star: "the STN's antialiased bilinear grid_sample fused with flow-compose in one pass".  The sampling grid is never
-// read from memory: every output pixel GENERATES its coordinate (and those of its 4 neighbours, for the level of detail)
-// from the head's raw regression outputs --
+// ---------------------------------------------------------------- the forward sampler
+// ONE kernel samples for every source of the grid.  MODE 0 reads each pixel's coordinate from an input grid (MipmapWarp,
+// Warp, grid_sample).  MODES 1 and 2 are the STN's sampling in one pass (north_star: "the STN's antialiased bilinear
+// grid_sample fused with flow-compose in one pass"): every output pixel GENERATES its coordinate (and those of its 4
+// neighbours, for the level of detail) from the head's raw regression outputs --
 //   MODE 1 (SimilarityHead, warping_heads.py:120-136): F.affine_grid(theta, align_corners=False): g = theta . [x, y, 1],
 //           x = (2*ox + 1)/Wo - 1
 //   MODE 2 (FlowHead, warping_heads.py:180-193,239-244,268-277): RAFT convex up-sampling (softmax over 9 mask logits x the 3x3
-//           neighbourhood of s*low_flow) + identity + apply_affine(base_warp) + alpha lerp
-// and then runs the level-of-detail / trilinear sampling of warp_fwd_kernel.  The grid (and the residual flow the TV
-// regulariser needs) are WRITTEN as by-products (the callers return them), replacing affine_grid (a bmm + 3 elementwise
-// launches) or the separate flow_compose pass and the grid read-back.
+//           neighbourhood of s*low_flow) + identity + apply_affine(base_warp) + alpha lerp (flow_compose.cuh)
+// and then runs the level-of-detail / trilinear sampling.  The generated grid (and the residual flow the TV regulariser
+// needs) are WRITTEN as by-products (the callers return them), replacing affine_grid (a bmm + 3 elementwise launches) or the
+// separate flow_compose pass and the grid read-back.
 struct ComposeParams {
+  const float* grid;      // MODE 0: (N, Ho, Wo, 2) sampling grid
   const float* theta;     // MODE 1: (N, 2, 3) sampling matrices.  MODE 2: base warp (N, 2, 3) or null
   const float* low;       // MODE 2: (N, lh, lw, 2)
   const float* mask;      // MODE 2: (N, 9*s*s, lh, lw)
   const float* identity;  // MODE 2: (s*lh, s*lw, 2) identity sampling grid (the head's buffer)
   const float* alpha;     // MODE 2: (N) or null
   int lh, lw, s;
-  float* grid_out;        // (N, Ho, Wo, 2) or null
+  float* grid_out;        // MODES 1, 2: (N, Ho, Wo, 2) or null
   float* delta_out;       // MODE 2: (N, Ho, Wo, 2) or null
 };
 
 template <int MODE>
 __device__ __forceinline__ float2 compose_at(const ComposeParams& cp, const WarpParams& p, int64_t n, int y, int x,
                                              float2* delta) {
-  if (MODE == 1) {
+  if (MODE == 0) {
+    return __ldg(reinterpret_cast<const float2*>(cp.grid + ((n * p.ho + y) * static_cast<int64_t>(p.wo) + x) * 2));
+  } else if (MODE == 1) {
     const float* M = cp.theta + n * 6;
     const float bx = (2.f * static_cast<float>(x) + 1.f) / static_cast<float>(p.wo) - 1.f;
     const float by = (2.f * static_cast<float>(y) + 1.f) / static_cast<float>(p.ho) - 1.f;
     return make_float2(fmaf(M[0], bx, fmaf(M[1], by, M[2])), fmaf(M[3], bx, fmaf(M[4], by, M[5])));
   } else {
     const int h = y / cp.s, w = x / cp.s, sy = y - h * cp.s, sx = x - w * cp.s;
-    float lg[9], mx = -INFINITY;
-#pragma unroll
-    for (int k = 0; k < 9; ++k) {
-      lg[k] = __ldg(cp.mask + ((((n * 9 + k) * cp.s + sy) * cp.s + sx) * cp.lh + h) * static_cast<int64_t>(cp.lw) + w);
-      mx = fmaxf(mx, lg[k]);
-    }
-    float sum = 0.f;
-#pragma unroll
-    for (int k = 0; k < 9; ++k) { lg[k] = expf(lg[k] - mx); sum += lg[k]; }
-    const float inv = 1.f / sum;
-    float dx = 0.f, dy = 0.f;
-#pragma unroll
-    for (int k = 0; k < 9; ++k) {
-      const int hh = h + k / 3 - 1, ww = w + k % 3 - 1;
-      if (hh >= 0 && hh < cp.lh && ww >= 0 && ww < cp.lw) {
-        const float2 f = __ldg(reinterpret_cast<const float2*>(cp.low + ((n * cp.lh + hh) * static_cast<int64_t>(cp.lw) + ww) * 2));
-        const float pk = lg[k] * inv;
-        dx = fmaf(pk, static_cast<float>(cp.s) * f.x, dx);
-        dy = fmaf(pk, static_cast<float>(cp.s) * f.y, dy);
-      }
-    }
-    if (delta) *delta = make_float2(dx, dy);
+    float pk[9], fx[9], fy[9];
+    const float2 u = convex_upsample(cp.low, cp.mask, n, cp.lh, cp.lw, cp.s, sy, sx, h, w, pk, fx, fy);
+    if (delta) *delta = u;
     const float2 id = __ldg(reinterpret_cast<const float2*>(cp.identity + (static_cast<int64_t>(y) * p.wo + x) * 2));
-    float gx = id.x + dx, gy = id.y + dy;
-    if (cp.theta) {
-      const float* M = cp.theta + n * 6;
-      const float tx = M[0] * gx + M[1] * gy + M[2];
-      const float ty = M[3] * gx + M[4] * gy + M[5];
-      gx = tx; gy = ty;
-    }
-    if (cp.alpha) {
-      const float a = __ldg(cp.alpha + n);
-      gx = id.x + a * (gx - id.x);
-      gy = id.y + a * (gy - id.y);
-    }
-    return make_float2(gx, gy);
+    return compose_flow(id, u.x, u.y, cp.theta, cp.alpha, n);
   }
 }
 
-// CTA = a 32 x 8 tile of output pixels of one sample.  Every thread generates the coordinate of ITS pixel once and parks it
-// in shared memory together with the one-pixel halo (computed by the first 84 threads), so the level of detail reads its 4
-// neighbours from shared memory instead of regenerating them (5x fewer softmax evaluations than a per-thread recompute).
+// CTA = a 32 x 8 tile of output pixels of one sample.  Every thread generates (MODE 0: reads) the coordinate of ITS pixel once
+// and parks it in shared memory together with the one-pixel halo (by the first 84 threads), so the level of detail reads its
+// 4 neighbours from shared memory instead of regenerating them (5x fewer softmax evaluations than a per-thread recompute).
 constexpr int kTileX = 32, kTileY = 8;
 
 template <typename T, bool MIP, int MODE>
@@ -476,8 +416,9 @@ warp_compose_fwd_kernel(T* __restrict__ out, float* __restrict__ levels_out, con
   int l0 = 0, l1 = 0;
   float w = 0.f;
   if (MIP) {
-    // (y, x) is replicate-clamped by the caller: a clamped neighbour of an edge pixel is the pixel itself or its in-tile
-    // neighbour; positions beyond the image but inside the tile hold clamped coordinates as well (computed above)
+    // level_of_detail replicate-clamps the neighbour indices to the image before it reads the tile, so it only reads live
+    // in-tile positions and the halo ring (which holds clamped coordinates, computed above); the out-of-image positions
+    // inside the tile (holding (0, 0)) are never read
     auto grid_at = [&](int y, int x) { return tile[y - y0 + 1][x - x0 + 1]; };
     const LevelInfo li = level_of_detail(grid_at, oy, ox, p.ho, p.wo, p.hs, p.ws, p.max_level, p.min_level);
     l0 = li.l0; l1 = li.l1; w = li.w;
@@ -518,18 +459,12 @@ mip_build_all_kernel(float* __restrict__ pyr, const T* __restrict__ src, const _
       float acc = 0.f;
 #pragma unroll
       for (int a = 0; a < 4; ++a) {
-        int yy = reflect_idx(2 * y + a - 1, in_h);
-        if (i == 1) yy = reflect_idx(yy - py.lp, py.hs);
+        const int yy = down_tap(2 * y + a - 1, in_h, i == 1, py.lp, py.hs);
 #pragma unroll
         for (int b = 0; b < 4; ++b) {
-          int xx = reflect_idx(2 * x + b - 1, in_w);
-          float v;
-          if (i == 1) {
-            xx = reflect_idx(xx - py.lp, py.ws);
-            v = Cvt<T>::to_f(src[(plane * py.hs + yy) * static_cast<int64_t>(py.ws) + xx]);
-          } else {
-            v = prev[yy * in_w + xx];
-          }
+          const int xx = down_tap(2 * x + b - 1, in_w, i == 1, py.lp, py.ws);
+          const float v = (i == 1) ? Cvt<T>::to_f(src[(plane * py.hs + yy) * static_cast<int64_t>(py.ws) + xx])
+                                   : prev[yy * in_w + xx];
           acc = fmaf(v, f[a] * f[b] * (1.f / 64.f), acc);
         }
       }
@@ -681,12 +616,6 @@ warp_bwd_kernel(float* __restrict__ grad_src, float* __restrict__ grad_pyr, floa
   }
 }
 
-inline int grid_for(int64_t total, int threads) {
-  int64_t g = (total + threads - 1) / threads;
-  const int64_t cap = static_cast<int64_t>(sm_count()) * 16;
-  return static_cast<int>(g < cap ? (g > 0 ? g : 1) : cap);
-}
-
 inline int fill_params(WarpParams* wp, int64_t n, int c, int hs, int ws, int ho, int wo, int pad_mode, int extra,
                        float max_level, float min_level) {
   if (n < 0 || c < 0 || hs < 1 || ws < 1 || ho < 0 || wo < 0) return fail(GG_ERR_BAD_ARG, "mipmap_warp: bad shape");
@@ -701,6 +630,33 @@ inline int fill_params(WarpParams* wp, int64_t n, int c, int hs, int ws, int ho,
   wp->max_level = max_level; wp->min_level = min_level;
   wp->lp = py.lp; wp->hp = py.hp; wp->wp = py.wp; wp->extra = extra;
   for (int i = 0; i <= kMaxLevels; ++i) wp->offset[i] = (i <= extra) ? py.offset[i] : 0;
+  return GG_OK;
+}
+
+// the forward sampler for every grid source: dtype x MIP x mode -> warp_compose_fwd_kernel
+template <typename T>
+void sample_t(void* out, float* levels_out, const void* src, const float* pyramid, const ComposeParams& cp,
+              const WarpParams& wp, int mode, unsigned ctas, int tiles_x, int tiles_y, cudaStream_t st) {
+  using Kernel = void (*)(T*, float*, const T*, const float*, const ComposeParams, const WarpParams, int, int);
+  const Kernel kernels[2][3] = {
+      {warp_compose_fwd_kernel<T, false, 0>, warp_compose_fwd_kernel<T, false, 1>, warp_compose_fwd_kernel<T, false, 2>},
+      {warp_compose_fwd_kernel<T, true, 0>, warp_compose_fwd_kernel<T, true, 1>, warp_compose_fwd_kernel<T, true, 2>}};
+  kernels[wp.extra > 0][mode]<<<ctas, kTileX * kTileY, 0, st>>>(static_cast<T*>(out), levels_out,
+                                                               static_cast<const T*>(src), pyramid, cp, wp, tiles_x, tiles_y);
+}
+
+int sample_forward(void* out, float* levels_out, const void* src, const float* pyramid, const ComposeParams& cp,
+                   const WarpParams& wp, int mode, int dtype, const char* who, cudaStream_t st) {
+  const int tiles_x = (wp.wo + kTileX - 1) / kTileX, tiles_y = (wp.ho + kTileY - 1) / kTileY;
+  const int64_t ctas = wp.n * tiles_x * static_cast<int64_t>(tiles_y);
+  if (ctas > 0x7fffffffLL) return fail(GG_ERR_BAD_ARG, "%s: too many tiles", who);
+  switch (dtype) {
+    case GG_F32: sample_t<float>(out, levels_out, src, pyramid, cp, wp, mode, ctas, tiles_x, tiles_y, st); break;
+    case GG_F16: sample_t<__half>(out, levels_out, src, pyramid, cp, wp, mode, ctas, tiles_x, tiles_y, st); break;
+    case GG_BF16: sample_t<__nv_bfloat16>(out, levels_out, src, pyramid, cp, wp, mode, ctas, tiles_x, tiles_y, st); break;
+    default: return fail(GG_ERR_UNSUPPORTED, "%s: dtype %d not supported", who, dtype);
+  }
+  GG_CHECK_LAUNCH("warp_compose_fwd launch");
   return GG_OK;
 }
 
@@ -816,24 +772,9 @@ int gg_mipmap_warp_forward(void* out, float* levels_out, const void* src, const 
   const int64_t total = N * ho * static_cast<int64_t>(wo);
   if (total == 0 || C == 0) return GG_OK;
   if (!out || !src || !grid || (extra_levels > 0 && !pyramid)) return fail(GG_ERR_BAD_ARG, "mipmap_warp_forward: null tensor");
-  auto st = static_cast<cudaStream_t>(stream);
-  const int gridsz = grid_for(total, 256);
-#define GG_FWD(T_)                                                                                               \
-  if (extra_levels > 0)                                                                                          \
-    warp_fwd_kernel<T_, true><<<gridsz, 256, 0, st>>>(static_cast<T_*>(out), levels_out, static_cast<const T_*>(src), \
-                                                      pyramid, grid, wp, total);                               \
-  else                                                                                                           \
-    warp_fwd_kernel<T_, false><<<gridsz, 256, 0, st>>>(static_cast<T_*>(out), levels_out, static_cast<const T_*>(src), \
-                                                       pyramid, grid, wp, total)
-  switch (dtype) {
-    case GG_F32: GG_FWD(float); break;
-    case GG_F16: GG_FWD(__half); break;
-    case GG_BF16: GG_FWD(__nv_bfloat16); break;
-    default: return fail(GG_ERR_UNSUPPORTED, "mipmap_warp_forward: dtype %d not supported", dtype);
-  }
-#undef GG_FWD
-  GG_CHECK_LAUNCH("warp_fwd launch");
-  return GG_OK;
+  ComposeParams cp{};
+  cp.grid = grid;
+  return sample_forward(out, levels_out, src, pyramid, cp, wp, 0, dtype, "mipmap_warp_forward", static_cast<cudaStream_t>(stream));
 }
 
 int gg_stn_sample_forward(void* out, float* grid_out, float* delta_out, float* levels_out, const void* src,
@@ -854,30 +795,10 @@ int gg_stn_sample_forward(void* out, float* grid_out, float* delta_out, float* l
     if (s < 1 || lh < 1 || lw < 1 || lh * s != ho || lw * s != wo)
       return fail(GG_ERR_BAD_ARG, "stn_sample: the flow grid (%d x %d, x%d) must match the output size (%d x %d)", lh, lw, s, ho, wo);
   }
-  ComposeParams cp;
+  ComposeParams cp{};
   cp.theta = theta; cp.low = low; cp.mask = mask; cp.identity = identity; cp.alpha = alpha;
   cp.lh = lh; cp.lw = lw; cp.s = s; cp.grid_out = grid_out; cp.delta_out = delta_out;
-  auto st = static_cast<cudaStream_t>(stream);
-  const int tiles_x = (wo + kTileX - 1) / kTileX, tiles_y = (ho + kTileY - 1) / kTileY;
-  const int64_t ctas = N * tiles_x * static_cast<int64_t>(tiles_y);
-  if (ctas > 0x7fffffffLL) return fail(GG_ERR_BAD_ARG, "stn_sample: too many tiles");
-  const unsigned gridsz = static_cast<unsigned>(ctas);
-#define GG_SS(T_, MIP_, MODE_)                                                                                   \
-  warp_compose_fwd_kernel<T_, MIP_, MODE_><<<gridsz, kTileX * kTileY, 0, st>>>(static_cast<T_*>(out), levels_out, \
-                                                                 static_cast<const T_*>(src), pyramid, cp, wp, tiles_x, tiles_y)
-#define GG_SS_T(T_)                                                                       \
-  if (extra_levels > 0) { if (mode == 1) GG_SS(T_, true, 1); else GG_SS(T_, true, 2); }   \
-  else { if (mode == 1) GG_SS(T_, false, 1); else GG_SS(T_, false, 2); }
-  switch (dtype) {
-    case GG_F32: GG_SS_T(float); break;
-    case GG_F16: GG_SS_T(__half); break;
-    case GG_BF16: GG_SS_T(__nv_bfloat16); break;
-    default: return fail(GG_ERR_UNSUPPORTED, "stn_sample: dtype %d not supported", dtype);
-  }
-#undef GG_SS_T
-#undef GG_SS
-  GG_CHECK_LAUNCH("warp_compose_fwd launch");
-  return GG_OK;
+  return sample_forward(out, levels_out, src, pyramid, cp, wp, mode, dtype, "stn_sample", static_cast<cudaStream_t>(stream));
 }
 
 int gg_mipmap_warp_backward(float* grad_src, float* grad_pyramid, float* grad_grid, const void* grad_out,

@@ -17,6 +17,7 @@ from torch.autograd import Function
 from torch.autograd.function import once_differentiable
 
 from .. import _lib
+from .flow import _f32c, flow_grads, flow_inputs, flow_meta
 
 
 def feasible_levels(h, w, wanted):
@@ -28,108 +29,50 @@ def feasible_levels(h, w, wanted):
     return e
 
 
-class _MipmapWarp(Function):
+def clamp_levels(hs, ws, max_num_levels, min_level):
+    """-> (max_level, min_level, extra): the requested levels of detail and the pyramid levels (beyond level 0) an hs x ws
+    source can host.  A tiny source cannot host them all; the reference only fails if such a level is actually selected,
+    so the levels are clamped to the feasible ones.  max_num_levels None: plain bilinear sampling."""
+    if max_num_levels is None:
+        return 0.0, 0.0, 0
+    max_level = float(max_num_levels) - 1.0
+    wanted = int(math.ceil(max(max_level, float(min_level), 0.0)))
+    extra = feasible_levels(hs, ws, wanted)
+    if extra < wanted:
+        max_level = min(max_level, float(extra))
+        min_level = min(float(min_level), float(extra))
+    return max_level, float(min_level), extra
+
+
+class _StnSample(Function):
+    """The [antialiased] sampler (csrc/warp.cu `warp_compose_fwd_kernel`), forward in one pass.  Mode 0 samples at a given
+    `grid`; modes 1 and 2 generate the grid inside the sampler from the STN head's raw outputs (mode 1: affine matrices
+    `theta`; mode 2: low-res flow + convex up-sampling mask [+ base warp `theta`, alpha]) and write it out as a by-product.
+    Backward = the sampler's backward on the (saved) grid, then the grid generator's (an einsum for the affine case, the
+    flow-composition kernel for the flow case)."""
+
     @staticmethod
-    def forward(ctx, inputs, grid, max_level, min_level, pad_mode, extra):
-        _lib.require_cuda(inputs, grid)
-        if inputs.dim() != 4 or grid.dim() != 4 or grid.shape[-1] != 2 or grid.shape[0] != inputs.shape[0]:
+    def forward(ctx, inputs, grid, theta, low, mask, identity, alpha, mode, out_hw, s, max_level, min_level, pad_mode, extra):
+        _lib.require_cuda(inputs, grid, theta, low, mask, identity, alpha)
+        if mode == 0 and (inputs.dim() != 4 or grid.dim() != 4 or grid.shape[-1] != 2 or grid.shape[0] != inputs.shape[0]):
             raise RuntimeError("warp: expected inputs (N, C, H, W) and grid (N, Ho, Wo, 2), got %s and %s" %
                                (tuple(inputs.shape), tuple(grid.shape)))
         lib = _lib.load()
         x = inputs.contiguous()
-        g = grid.float().contiguous()
         n, c, hs, ws = x.shape
-        ho, wo = g.shape[1], g.shape[2]
         code = _lib.dtype_code(x)
         st = _lib.stream()
-        pyr = None
-        if extra > 0:
-            elems = lib.gg_mipmap_pyramid_elems(n * c, hs, ws, extra)
-            if elems < 0:
-                raise RuntimeError("MipmapWarp: a %dx%d source cannot host %d mip levels" % (hs, ws, extra))
-            pyr = torch.empty(max(int(elems), 1), dtype=torch.float32, device=x.device)
-            _lib.check(lib.gg_mipmap_build(pyr.data_ptr(), x.data_ptr(), code, n * c, hs, ws, extra, st), "gg_mipmap_build")
-        out = torch.empty((n, c, ho, wo), dtype=x.dtype, device=x.device)
-        levels = torch.empty((n, ho, wo), dtype=torch.float32, device=x.device) if extra > 0 else None
-        rc = lib.gg_mipmap_warp_forward(out.data_ptr(), _lib.ptr(levels), x.data_ptr(), _lib.ptr(pyr), g.data_ptr(), code,
-                                        n, c, hs, ws, ho, wo, extra, max_level, min_level, pad_mode, st)
-        _lib.check(rc, "gg_mipmap_warp_forward")
-        ctx.save_for_backward(x, g, pyr)
-        ctx.cfg = (max_level, min_level, pad_mode, extra, grid.dtype)
-        if levels is None:
-            levels = out.new_zeros(())
-        ctx.mark_non_differentiable(levels)
-        return out, levels
-
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, grad_out, _grad_levels):
-        x, g, pyr = ctx.saved_tensors
-        max_level, min_level, pad_mode, extra, grid_dtype = ctx.cfg
-        need_x, need_g = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
-        lib = _lib.load()
-        n, c, hs, ws = x.shape
-        ho, wo = g.shape[1], g.shape[2]
-        st = _lib.stream()
-        go = grad_out.contiguous()
-        if go.dtype != x.dtype:
-            go = go.to(x.dtype)
-        grad_src = torch.zeros(x.shape, dtype=torch.float32, device=x.device) if need_x else None
-        grad_pyr = torch.zeros_like(pyr) if (need_x and pyr is not None) else None
-        grad_grid = torch.zeros(g.shape, dtype=torch.float32, device=x.device) if need_g else None
-        rc = lib.gg_mipmap_warp_backward(_lib.ptr(grad_src), _lib.ptr(grad_pyr), _lib.ptr(grad_grid), go.data_ptr(),
-                                         x.data_ptr(), _lib.ptr(pyr), g.data_ptr(), _lib.dtype_code(x), n, c, hs, ws,
-                                         ho, wo, extra, max_level, min_level, pad_mode, st)
-        _lib.check(rc, "gg_mipmap_warp_backward")
-        if need_x and extra > 0:
-            rc = lib.gg_mipmap_build_backward(grad_src.data_ptr(), grad_pyr.data_ptr(), n * c, hs, ws, extra, st)
-            _lib.check(rc, "gg_mipmap_build_backward")
-        if grad_src is not None and grad_src.dtype != x.dtype:
-            grad_src = grad_src.to(x.dtype)
-        if grad_grid is not None and grad_grid.dtype != grid_dtype:
-            grad_grid = grad_grid.to(grid_dtype)
-        return grad_src, grad_grid, None, None, None, None
-
-
-class _StnSample(Function):
-    """The STN's sampling in one forward pass (csrc/warp.cu `warp_compose_fwd_kernel`): the sampling grid is generated
-    inside the sampler from the head's raw outputs (mode 1: affine matrices; mode 2: low-res flow + convex up-sampling mask
-    [+ base warp, alpha]) and written out as a by-product.  Backward = the sampler's backward on the saved grid, then the
-    grid generator's (an einsum for the affine case, the flow-composition kernel for the flow case)."""
-
-    @staticmethod
-    def forward(ctx, inputs, theta, low, mask, identity, alpha, mode, out_hw, s, max_level, min_level, pad_mode, extra):
-        _lib.require_cuda(inputs, theta, low, mask, identity, alpha)
-        lib = _lib.load()
-        x = inputs.contiguous()
-        n, c, hs, ws = x.shape
-        ho, wo = out_hw
-        code = _lib.dtype_code(x)
-        st = _lib.stream()
-
-        def f32(t):
-            if t is None:
-                return None
-            t = t.detach()
-            return t if (t.dtype == torch.float32 and t.is_contiguous()) else t.float().contiguous()
-        th, lo, mk, idn, al = f32(theta), f32(low), f32(mask), f32(identity), f32(alpha)
-        lh = lw = 0
+        flow_in = (None,) * 5
+        th = None
         if mode == 2:
-            if lo.dim() != 4 or lo.shape[0] != n or lo.shape[-1] != 2:
+            if low.dim() != 4 or low.shape[0] != n:
                 raise RuntimeError("stn_sample: low-res flow must be (N, h, w, 2) with N = the image batch")
-            lh, lw = lo.shape[1], lo.shape[2]
-            if mk.numel() != n * 9 * s * s * lh * lw or idn.numel() != ho * wo * 2:
-                raise RuntimeError("stn_sample: mask must be (N, 9*s*s, h, w) and identity_flow (1, s*h, s*w, 2)")
-            if al is not None:
-                al = al.reshape(-1)
-                if al.numel() == 1:
-                    al = al.expand(n).contiguous()
-                elif al.numel() != n:
-                    raise RuntimeError("stn_sample: alpha must have 1 or N elements")
-            if th is not None and th.numel() != n * 6:
-                raise RuntimeError("stn_sample: base_warp must be (N, 2, 3)")
-        elif th is None or th.numel() != n * 6:
-            raise RuntimeError("stn_sample: theta must be (N, 2, 3)")
+            flow_in = flow_inputs("stn_sample", low, mask, identity, theta, alpha, s)
+            th = flow_in[3]
+        elif mode == 1:
+            th = _f32c(theta)
+            if th is None or th.numel() != n * 6:
+                raise RuntimeError("stn_sample: theta must be (N, 2, 3)")
         pyr = None
         if extra > 0:
             elems = lib.gg_mipmap_pyramid_elems(n * c, hs, ws, extra)
@@ -137,36 +80,42 @@ class _StnSample(Function):
                 raise RuntimeError("MipmapWarp: a %dx%d source cannot host %d mip levels" % (hs, ws, extra))
             pyr = torch.empty(max(int(elems), 1), dtype=torch.float32, device=x.device)
             _lib.check(lib.gg_mipmap_build(pyr.data_ptr(), x.data_ptr(), code, n * c, hs, ws, extra, st), "gg_mipmap_build")
+        ho, wo = (grid.shape[1], grid.shape[2]) if mode == 0 else out_hw
         out = torch.empty((n, c, ho, wo), dtype=x.dtype, device=x.device)
-        grid = torch.empty((n, ho, wo, 2), dtype=torch.float32, device=x.device)
-        delta = torch.empty((n, ho, wo, 2), dtype=torch.float32, device=x.device) if mode == 2 else None
         levels = torch.empty((n, ho, wo), dtype=torch.float32, device=x.device) if extra > 0 else None
-        rc = lib.gg_stn_sample_forward(out.data_ptr(), grid.data_ptr(), _lib.ptr(delta), _lib.ptr(levels), x.data_ptr(),
-                                       _lib.ptr(pyr), _lib.ptr(th), _lib.ptr(lo), _lib.ptr(mk), _lib.ptr(idn), _lib.ptr(al),
-                                       mode, code, n, c, hs, ws, ho, wo, lh, lw, s, extra, max_level, min_level, pad_mode, st)
-        _lib.check(rc, "gg_stn_sample_forward")
-        ctx.save_for_backward(x, grid, pyr, th, lo, mk, idn, al)
-        ctx.cfg = (mode, s, max_level, min_level, pad_mode, extra,
-                   None if theta is None else (theta.dtype, tuple(theta.shape)),
-                   None if low is None else low.dtype, None if mask is None else (mask.dtype, tuple(mask.shape)))
-        if delta is None:
-            delta = out.new_zeros(())
-        if levels is None:
-            levels = out.new_zeros(())
-        ctx.mark_non_differentiable(levels)
-        return out, grid, delta, levels
+        delta = None
+        if mode == 0:
+            g = _f32c(grid)
+            rc = lib.gg_mipmap_warp_forward(out.data_ptr(), _lib.ptr(levels), x.data_ptr(), _lib.ptr(pyr), g.data_ptr(), code,
+                                            n, c, hs, ws, ho, wo, extra, max_level, min_level, pad_mode, st)
+            _lib.check(rc, "gg_mipmap_warp_forward")
+        else:
+            g = torch.empty((n, ho, wo, 2), dtype=torch.float32, device=x.device)
+            delta = torch.empty((n, ho, wo, 2), dtype=torch.float32, device=x.device) if mode == 2 else None
+            lo, mk, idn, _, al = flow_in
+            lh, lw = (lo.shape[1], lo.shape[2]) if mode == 2 else (0, 0)
+            rc = lib.gg_stn_sample_forward(out.data_ptr(), g.data_ptr(), _lib.ptr(delta), _lib.ptr(levels), x.data_ptr(),
+                                           _lib.ptr(pyr), _lib.ptr(th), _lib.ptr(lo), _lib.ptr(mk), _lib.ptr(idn), _lib.ptr(al),
+                                           mode, code, n, c, hs, ws, ho, wo, lh, lw, s, extra, max_level, min_level, pad_mode, st)
+            _lib.check(rc, "gg_stn_sample_forward")
+        ctx.save_for_backward(x, g, pyr, *flow_in)
+        ctx.cfg = (mode, s, max_level, min_level, pad_mode, extra, None if grid is None else grid.dtype,
+                   None if theta is None else (theta.dtype, tuple(theta.shape)), flow_meta(low, mask, theta) if mode == 2 else None)
+        if levels is not None:
+            ctx.mark_non_differentiable(levels)
+        return out, (None if mode == 0 else g), delta, levels   # None: an output this mode does not have
 
     @staticmethod
     @once_differentiable
     def backward(ctx, g_out, g_grid, g_delta, _g_levels):
-        x, grid, pyr, th, lo, mk, idn, al = ctx.saved_tensors
-        mode, s, max_level, min_level, pad_mode, extra, theta_info, low_dt, mask_info = ctx.cfg
-        need_x, need_theta, need_low, need_mask = ctx.needs_input_grad[:4]
+        x, grid, pyr, *flow_in = ctx.saved_tensors
+        mode, s, max_level, min_level, pad_mode, extra, grid_dtype, theta_info, flow_like = ctx.cfg
+        need_x, need_grid_in, need_theta, need_low, need_mask = ctx.needs_input_grad[:5]
         lib = _lib.load()
         n, c, hs, ws = x.shape
         ho, wo = grid.shape[1], grid.shape[2]
         st = _lib.stream()
-        need_grid = need_theta or need_low or need_mask
+        need_grid = need_grid_in or need_theta or need_low or need_mask
         grad_src = torch.zeros(x.shape, dtype=torch.float32, device=x.device) if need_x else None
         grad_pyr = torch.zeros_like(pyr) if (need_x and pyr is not None) else None
         gg = None
@@ -182,10 +131,13 @@ class _StnSample(Function):
             if need_x and extra > 0:
                 _lib.check(lib.gg_mipmap_build_backward(grad_src.data_ptr(), grad_pyr.data_ptr(), n * c, hs, ws, extra, st),
                            "gg_mipmap_build_backward")
-        if need_grid and g_grid is not None and g_grid.dim() == 4:     # the caller also used the returned grid
+        if need_grid and g_grid is not None:     # the caller also used the returned grid
             gg = g_grid.float().contiguous() if gg is None else gg + g_grid.float()
-        g_theta = g_low = g_mask = None
-        if mode == 1:
+        g_grid_in = g_theta = g_low = g_mask = None
+        if mode == 0:
+            if need_grid_in and gg is not None:
+                g_grid_in = gg if gg.dtype == grid_dtype else gg.to(grid_dtype)
+        elif mode == 1:
             if need_theta and gg is not None:
                 # grid = [bx, by, 1] . theta^T  ->  d theta[n, i, k] = sum_yx gg[n, y, x, i] * base[y, x, k]
                 bx = (2.0 * torch.arange(wo, device=x.device, dtype=torch.float32) + 1.0) / wo - 1.0
@@ -193,61 +145,32 @@ class _StnSample(Function):
                 g_theta = torch.stack([torch.einsum("nyxi,x->ni", gg, bx), torch.einsum("nyxi,y->ni", gg, by), gg.sum(dim=(1, 2))], dim=2)
                 g_theta = g_theta.reshape(theta_info[1]).to(theta_info[0])
         else:
-            gd = g_delta.float().contiguous() if (g_delta is not None and g_delta.dim() == 4) else None
+            gd = g_delta.float().contiguous() if g_delta is not None else None
             if (need_low or need_mask or need_theta) and (gg is not None or gd is not None):
-                g_mask = torch.empty_like(mk) if need_mask else None
-                g_low = torch.zeros_like(lo) if need_low else None
-                g_base = torch.zeros((n, 2, 3), dtype=torch.float32, device=x.device) if (need_theta and th is not None) else None
-                lh, lw = lo.shape[1], lo.shape[2]
-                rc = lib.gg_flow_compose_backward(_lib.ptr(g_mask), _lib.ptr(g_low), _lib.ptr(g_base), _lib.ptr(gd), _lib.ptr(gg),
-                                                  lo.data_ptr(), mk.data_ptr(), _lib.ptr(idn), _lib.ptr(th), _lib.ptr(al),
-                                                  n, lh, lw, s, st)
-                _lib.check(rc, "gg_flow_compose_backward")
-                if g_mask is not None:
-                    g_mask = g_mask.reshape(mask_info[1]).to(mask_info[0])
-                if g_low is not None:
-                    g_low = g_low.to(low_dt)
-                if g_base is not None:
-                    g_theta = g_base.reshape(theta_info[1]).to(theta_info[0])
+                g_low, g_mask, g_theta = flow_grads(flow_in, flow_like, s, gd, gg, need_low, need_mask, need_theta)
         if grad_src is not None and grad_src.dtype != x.dtype:
             grad_src = grad_src.to(x.dtype)
-        return (grad_src, g_theta, g_low, g_mask) + (None,) * 9
-
-
-def _levels_for(inputs, max_num_levels, min_level):
-    max_level = float(max_num_levels) - 1.0
-    wanted = int(math.ceil(max(max_level, float(min_level), 0.0)))
-    extra = feasible_levels(inputs.shape[2], inputs.shape[3], wanted)
-    if extra < wanted:
-        max_level = min(max_level, float(extra))
-        min_level = min(float(min_level), float(extra))
-    return max_level, float(min_level), extra
+        return (grad_src, g_grid_in, g_theta, g_low, g_mask) + (None,) * 9
 
 
 def stn_sample_affine(inputs, theta, out_hw, max_num_levels=None, min_level=0.0, padding_mode="border"):
     """F.affine_grid(theta, align_corners=False) + [antialiased] bilinear sampling of `inputs`, one pass.
     max_num_levels None: plain `Warp`.  -> (out, grid (N, Ho, Wo, 2), levels or None)."""
-    if max_num_levels is None:
-        max_level, min_level, extra = 0.0, 0.0, 0
-    else:
-        max_level, min_level, extra = _levels_for(inputs, max_num_levels, min_level)
-    out, grid, _, levels = _StnSample.apply(inputs, theta, None, None, None, None, 1, tuple(out_hw), 1, max_level, min_level,
-                                            _pad_code(padding_mode), extra)
-    return out, grid, (levels if extra > 0 else None)
+    max_level, min_level, extra = clamp_levels(inputs.shape[2], inputs.shape[3], max_num_levels, min_level)
+    out, grid, _, levels = _StnSample.apply(inputs, None, theta, None, None, None, None, 1, tuple(out_hw), 1, max_level,
+                                            min_level, _pad_code(padding_mode), extra)
+    return out, grid, levels
 
 
 def stn_sample_flow(inputs, low, mask, identity_flow, base_warp, alpha, downsample, max_num_levels=None, min_level=0.0,
                     padding_mode="border"):
     """FlowHead's upsample_flow + identity + apply_affine + alpha lerp (warping_heads.py:180-193,239-244,268-277) generated
     inside the [antialiased] sampler, one pass.  -> (out, flow (N, sH, sW, 2), delta_flow (N, sH, sW, 2), levels or None)."""
-    if max_num_levels is None:
-        max_level, min_level, extra = 0.0, 0.0, 0
-    else:
-        max_level, min_level, extra = _levels_for(inputs, max_num_levels, min_level)
+    max_level, min_level, extra = clamp_levels(inputs.shape[2], inputs.shape[3], max_num_levels, min_level)
     ho, wo = low.shape[1] * downsample, low.shape[2] * downsample
-    out, grid, delta, levels = _StnSample.apply(inputs, base_warp, low, mask, identity_flow, alpha, 2, (ho, wo), int(downsample),
-                                                max_level, min_level, _pad_code(padding_mode), extra)
-    return out, grid, delta, (levels if extra > 0 else None)
+    out, grid, delta, levels = _StnSample.apply(inputs, None, base_warp, low, mask, identity_flow, alpha, 2, (ho, wo),
+                                                int(downsample), max_level, min_level, _pad_code(padding_mode), extra)
+    return out, grid, delta, levels
 
 
 def sample_indices(grid, source_hw, max_num_levels=8, min_level=0.0, padding_mode="border"):
@@ -256,11 +179,7 @@ def sample_indices(grid, source_hw, max_num_levels=8, min_level=0.0, padding_mod
     detail, from the device functions the sampling kernels use (gg_warp_sample_indices; for exact parity tests)."""
     _lib.require_cuda(grid)
     hs, ws = int(source_hw[0]), int(source_hw[1])
-    max_level = float(max_num_levels) - 1.0
-    wanted = int(math.ceil(max(max_level, float(min_level), 0.0)))
-    extra = feasible_levels(hs, ws, wanted)
-    if extra < wanted:
-        max_level, min_level = min(max_level, float(extra)), min(float(min_level), float(extra))
+    max_level, min_level, _ = clamp_levels(hs, ws, max_num_levels, min_level)
     g = grid.detach().float().contiguous()
     n, ho, wo, _ = g.shape
     out = torch.empty(n, ho, wo, 4, dtype=torch.int32, device=g.device)
@@ -279,14 +198,10 @@ def _pad_code(padding_mode):
 
 def mipmap_warp(inputs, grid, max_num_levels=8, min_level=0.0, padding_mode="border"):
     """Functional form of MipmapWarp.forward: -> (outputs, levels (N, Ho, Wo) fp32)."""
-    max_level = float(max_num_levels) - 1.0
-    wanted = int(math.ceil(max(max_level, float(min_level), 0.0)))
-    extra = feasible_levels(inputs.shape[2], inputs.shape[3], wanted)
-    if extra < wanted:  # tiny source: the reference only fails if such a level is actually selected
-        max_level = min(max_level, float(extra))
-        min_level = min(float(min_level), float(extra))
-    out, levels = _MipmapWarp.apply(inputs, grid, max_level, float(min_level), _pad_code(padding_mode), extra)
-    if extra == 0:
+    max_level, min_level, extra = clamp_levels(inputs.shape[2], inputs.shape[3], max_num_levels, min_level)
+    out, _, _, levels = _StnSample.apply(inputs, grid, None, None, None, None, None, 0, None, 1, max_level, min_level,
+                                         _pad_code(padding_mode), extra)
+    if levels is None:
         levels = torch.zeros(grid.shape[:3], device=grid.device)
     return out, levels
 
@@ -341,7 +256,7 @@ def bilinear_downsample(input, stride, kernel_horz, kernel_vert):
 
 def grid_sample_bilinear(inputs, grid, padding_mode="border"):
     """F.grid_sample(inputs, grid, padding_mode=..., align_corners=False) through the fused kernel (no mip levels)."""
-    return _MipmapWarp.apply(inputs, grid, 0.0, 0.0, _pad_code(padding_mode), 0)[0]
+    return _StnSample.apply(inputs, grid, None, None, None, None, None, 0, None, 1, 0.0, 0.0, _pad_code(padding_mode), 0)[0]
 
 
 def _default_ops():

@@ -174,7 +174,7 @@ GG_API int gg_mipmap_warp_backward(float* grad_src, float* grad_pyramid, float* 
 /* The sampler's INTEGER work, exported for exact parity tests (no reference counterpart: ATen's grid_sampler_2d and
  * antialiased_sampling.py:228-229 compute these integers internally).  indices: int32 (N, Ho, Wo, 4), 16-byte aligned =
  * (x0, y0, l0, l1): north-west bilinear corner after the padding-mode transform, floor / ceil of the level of detail --
- * evaluated by the same device functions as gg_mipmap_warp_forward / gg_stn_sample_forward. */
+ * evaluated by the same device functions as the forward sampler of gg_mipmap_warp_forward / gg_stn_sample_forward. */
 GG_API int gg_warp_sample_indices(int32_t* indices, const float* grid, int64_t N, int hs, int ws, int ho, int wo,
                                   float max_level, float min_level, int padding_mode, void* stream);
 
@@ -221,8 +221,9 @@ GG_API int gg_splat2d_forward(float* out, void* workspace, const float* input, c
  *   mode 2  FlowHead (warping_heads.py:180-193 upsample_flow, :239-244, :268-277 apply_affine): low (N, lh, lw, 2),
  *           mask (N, 9*s*s, lh, lw), identity (s*lh, s*lw, 2), optional base warp `theta` (N, 2, 3) and alpha (N);
  *           ho == s*lh, wo == s*lw
- * then the level-of-detail selection + trilinear sample of gg_mipmap_warp_forward (antialiased_sampling.py:35-238) on
- * `src` (N, C, hs, ws) and its `pyramid` (gg_mipmap_build; extra_levels == 0: plain bilinear sampling).
+ * then the level-of-detail selection + trilinear sample of gg_mipmap_warp_forward (antialiased_sampling.py:35-238; the
+ * same kernel, which there reads the grid) on `src` (N, C, hs, ws) and its `pyramid` (gg_mipmap_build; extra_levels == 0:
+ * plain bilinear sampling).
  * Outputs: out (N, C, ho, wo); grid_out (N, ho, wo, 2) and delta_out (mode 2: the residual flow of the TV regulariser,
  * reference models/losses/loss.py:4-12) are written as by-products (NULL: skipped); levels_out (N, ho, wo) or NULL.
  * The backward pass is gg_mipmap_warp_backward on grid_out (+ gg_flow_compose_backward for mode 2).

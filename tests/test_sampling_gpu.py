@@ -430,7 +430,7 @@ def test_sampler_integer_work_is_bit_exact(mode, hs, ws):
 # ------------------------------------------------------------------------------------------------ one-pass STN sampler
 def grid_stride_batch(ho, wo):
     """A batch whose N * Ho * Wo output pixels exceed one trip of the sampler's grid-stride loops (16 CTAs of 256 threads
-    per SM: csrc/warp.cu grid_for, csrc/flow.cu flow_grid), so that every thread makes a second trip."""
+    per SM: csrc/flow_compose.cuh grid_for), so that every thread makes a second trip."""
     from gangealing_b200 import _lib
     return _lib.sm_count() * 16 * 256 // (ho * wo) + 2
 
@@ -586,3 +586,58 @@ def test_stn_sample_beyond_the_grid_stride_cap():
     n = grid_stride_batch(128, 128)
     _check_stn_affine(n, (128, 128), 4, "border", torch.float32, seed=1)
     _check_stn_flow(n, 16, 16, 8, True, "n", 4, "border", torch.float32, seed=1)
+
+
+@pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16])
+@pytest.mark.parametrize("mode", S.PAD_MODES)
+@pytest.mark.parametrize("levels", [None, 4])
+@pytest.mark.parametrize("out_hw", [(128, 128), (100, 60), (7, 300), (1, 1)])
+def test_one_sampler_for_given_and_generated_grids(out_hw, levels, mode, dtype):
+    """One forward kernel samples every grid: mipmap_warp (Warp and grid_sample_bilinear without levels) on the grid that
+    stn_sample_affine generated reproduce its output and level map bit for bit.  The odd sizes overhang the 32x8 tiles of
+    a read grid, and (1, 1) clamps every neighbour onto the pixel itself."""
+    stn = _stn()
+    from gangealing_b200.stn import sampling as GS
+    g = torch.Generator().manual_seed(out_hw[0] * 1000 + out_hw[1])
+    n = 3
+    x = torch.randn(n, 3, 128, 128, generator=g).to(dtype).to(DEV)
+    theta = torch.eye(2, 3)[None] * (0.5 + 1.5 * torch.rand(n, 1, 1, generator=g)) + 0.15 * torch.randn(n, 2, 3, generator=g)
+    with torch.no_grad():
+        out, grid, lv = GS.stn_sample_affine(x, theta.to(DEV), out_hw, levels, 0.0, mode)
+        if levels is None:
+            assert torch.equal(stn.Warp()(x, grid, mode), out)
+            assert torch.equal(GS.grid_sample_bilinear(x, grid, mode), out)
+        else:
+            out_g, lv_g = GS.mipmap_warp(x, grid, levels, 0.0, mode)
+            assert torch.equal(out_g, out)
+            assert torch.equal(lv_g, lv)
+
+
+@pytest.mark.parametrize("lh,lw,s,with_base,alpha,levels,mode", FLOW_CASES)
+def test_one_flow_composition_for_op_and_sampler(lh, lw, s, with_base, alpha, levels, mode):
+    """The stand-alone flow_compose and the one-pass flow sampler compose the same grid bit for bit, and sampling that grid
+    with mipmap_warp (grid_sample_bilinear without levels) reproduces the one-pass output and level map."""
+    from gangealing_b200.stn import flow as GF
+    from gangealing_b200.stn import sampling as GS
+    g = torch.Generator().manual_seed(lh * 100 + lw + s)
+    n = 3
+    ho, wo = lh * s, lw * s
+    hs = ws = 128 if s > 1 else 32
+    x = torch.randn(n, 3, hs, ws, generator=g).to(DEV)
+    low = ((0.1 / s) * torch.randn(n, lh, lw, 2, generator=g)).to(DEV)
+    mask = (2.0 * torch.randn(n, 9 * s * s, lh, lw, generator=g)).to(DEV)
+    base = (torch.eye(2, 3)[None] * 1.4 + 0.1 * torch.randn(n, 2, 3, generator=g)).to(DEV) if with_base else None
+    alpha = {None: None, "n": torch.rand(n, generator=g), "1": torch.rand(1, generator=g)}[alpha]
+    alpha = None if alpha is None else alpha.to(DEV)
+    ident = S.affine_grid_ref(torch.eye(2, 3)[None], (1, 1, ho, wo)).to(DEV)
+    with torch.no_grad():
+        out, flow, delta, lv = GS.stn_sample_flow(x, low, mask, ident, base, alpha, s, levels, 0.0, mode)
+        delta_c, flow_c = GF.flow_compose(low, mask, ident, base, alpha, s)
+        assert torch.equal(delta_c, delta)
+        assert torch.equal(flow_c, flow)
+        if levels is None:
+            assert torch.equal(GS.grid_sample_bilinear(x, flow, mode), out)
+        else:
+            out_g, lv_g = GS.mipmap_warp(x, flow, levels, 0.0, mode)
+            assert torch.equal(out_g, out)
+            assert torch.equal(lv_g, lv)

@@ -80,6 +80,7 @@ SIGNATURES = {
     "gg_tv_per_sample": (_I, [_P, _P, _L, _I, _I, _P]),
     "gg_pck_transfer_workspace": (_L, [_L, _L, _I]),
     "gg_pck_transfer": (_I, [_P] * 14 + [_L, _L, _I, _I, _I, _I, _I, _P]),
+    "gg_batch_gram": (_I, [_P, _P, _P, _P, _L, _I, _P]),
 }
 
 _dll = None

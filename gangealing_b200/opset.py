@@ -24,6 +24,7 @@ def cuda_ops():
         from .op import feature_distance as _fd
         from .op import vgg_pool as _vp
         from .evaluation import ops as _ev
+        from .op import pca as _pca
         _cached = types.SimpleNamespace(
             name="sm_90a",
             upfirdn2d=_op.upfirdn2d,
@@ -51,5 +52,6 @@ def cuda_ops():
             bias_relu_pool_supported=_vp.supported,
             tv_per_sample=_ev.tv_per_sample,              # match_flows / flow_scores: per-sample smoothness, one launch
             pck_transfer_points=_ev.pck_transfer_points,  # PCK-Transfer: congeal + search + lookup + score, one call
+            batch_gram=_pca.batch_gram,                   # IncrementalPCA's per-batch means + centred Grams, fp64 DMMA
         )
     return _cached

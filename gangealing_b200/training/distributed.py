@@ -54,6 +54,11 @@ def all_gather(tensor, cat=True):
     return torch.cat(out, 0) if cat else out
 
 
+def rank0_to_all(tensor):
+    """Rank 0's value of `tensor` on every rank (reference distributed.py:134-137)."""
+    return all_gather(tensor)[0]
+
+
 def all_reduce_mean(tensor):
     if get_world_size() == 1:
         return tensor

@@ -13,7 +13,7 @@ from torch import nn, optim
 from ..stn import BilinearDownsample, get_stn
 from ..stylegan2 import Generator
 from . import distributed as gdist
-from .latent_learner import DirectionInterpolator
+from .latent_learner import PCA, DirectionInterpolator, kmeans_plusplus
 from .losses import flow_identity_loss, gangealing_cluster_loss, gangealing_loss, total_variation_loss
 from .perceptual import get_perceptual_loss
 
@@ -75,7 +75,7 @@ class Trainer:
     `ops`: None = the sm_90a op set; tests/bench's CPU legs pass the oracle's."""
 
     def __init__(self, cfg, device, ops=None, distributed=False, seed_offset=0):
-        self.cfg, self.device, self.distributed = cfg, device, distributed
+        self.cfg, self.device, self.distributed, self.ops = cfg, device, distributed, ops
         torch.manual_seed(cfg.seed)  # identical weights on every rank (stands in for the shared checkpoint)
         self.generator = Generator(cfg.gen_size, cfg.dim_latent, cfg.n_mlp, channel_multiplier=cfg.gen_channel_multiplier,
                                    ops=ops).to(device).eval()
@@ -263,6 +263,30 @@ class Trainer:
         if ckpt.get("iteration") is not None:
             self.set_iteration(int(ckpt["iteration"]))
         return True
+
+    @torch.no_grad()
+    def init_target_mode(self, n_pca=1_000_000, n_kmeans=50_000, debug=False):
+        """Initialise the latent learner from the generator, as reference train.py:228-243 does after loading only
+        `g_ema`: an IncrementalPCA of n_pca generated latents (n_pca // world per rank, all-gathered) gives `directions`
+        and `lat_mean`; with several heads, k-means++ over n_kmeans latents (or, with `debug`, num_heads random latents)
+        gives the centroids whose PCA codes become `coefficients`.  `debug` also sets n_pca = 1000.
+        The three tensors are written in place: the fused optimiser's pointer table and a captured graph stay valid.
+        -> the fitted PCA."""
+        cfg = self.cfg
+        if debug:
+            n_pca = 1000
+        batch_w = gdist.all_gather(self.generator.batch_latent(n_pca // gdist.get_world_size()))
+        pca = PCA(cfg.ndirs, batch_w, ops=self.ops)
+        ll = self.ll_module
+        ll.directions.copy_(torch.from_numpy(pca.components_).float())
+        ll.lat_mean.copy_(torch.from_numpy(pca.mean_[None]).float())
+        if cfg.num_heads > 1:
+            if debug:
+                centroids = self.generator.batch_latent(cfg.num_heads)
+            else:
+                centroids = kmeans_plusplus(cfg.num_heads, n_kmeans, self.generator, self.loss_fn, cfg.inject)
+            ll.assign_coefficients(pca.encode(centroids))
+        return pca
 
     def step(self, z=None, psi=None, lr=None, ll_lr=None):
         """-> dict of (rank-0 averaged) scalar loss tensors, still on the device (no host sync here).

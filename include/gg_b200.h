@@ -468,6 +468,18 @@ GG_API int gg_tv_loss_backward(float* grad_flow, const float* grad_out, const fl
 GG_API int gg_scale_cast_multi(const void* table, const int* block_tensor, const int* block_chunk, int blocks, int chunk,
                                void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Latent-learner initialisation, csrc/pca.cu: the per-batch terms of IncrementalPCA's Gram form
+ * (gangealing_b200/training/latent_learner.py; reference models/latent_learner.py:8-22).
+ *   gg_batch_gram: for each of the B row blocks [batch_offsets[b], batch_offsets[b+1]) of the row-major fp32 (n, D) matrix w
+ *     (DEVICE, 16-byte aligned): mean (B, D) fp64 the block's column mean (fixed summation order) and gram (B, D, D) fp64
+ *     the full symmetric sum over its rows of (x - mean_b)(x - mean_b)^T, on the fp64 tensor cores (DMMA).  batch_offsets:
+ *     HOST int64 array of B + 1 entries, offsets[0] >= 0, strictly increasing (GG_ERR_BAD_ARG otherwise); D a multiple of
+ *     64 and at most 1024 (GG_ERR_UNSUPPORTED otherwise).  No atomics (bitwise reproducible), no sync, no allocation.
+ * ---------------------------------------------------------------------------------------------- */
+GG_API int gg_batch_gram(double* gram, double* mean, const float* w, const int64_t* batch_offsets, int64_t B, int D,
+                         void* stream);
+
 #ifdef __cplusplus
 }
 #endif

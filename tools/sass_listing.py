@@ -6,7 +6,7 @@
 Runs `cuobjdump -sass` on gangealing_b200/libgg_b200.so (no GPU needed) and prints, for every kernel, the count of the
 Hopper-specific / memory-path mnemonics that show wgmma / TMA / bulk-copy use:
 
-  HGMMA (wgmma.mma_async), UTMALDG (cp.async.bulk.tensor = TMA tensor map),
+  HGMMA (wgmma.mma_async), DMMA (fp64 mma.sync), UTMALDG (cp.async.bulk.tensor = TMA tensor map),
   UBLKCP (cp.async.bulk = 1-D bulk TMA), SYNCS (mbarrier), REDG (red.global), MATCH (match.any),
   LDG/STG.E.128 and LDS.128 (16-byte accesses), plus register count per kernel from `cuobjdump -res-usage`.
 """
@@ -18,7 +18,7 @@ import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-MNEMONICS = ["HGMMA", "UTMALDG", "UBLKCP", "SYNCS", "REDG", "MATCH", "LDG.E.128", "STG.E.128",
+MNEMONICS = ["HGMMA", "DMMA", "UTMALDG", "UBLKCP", "SYNCS", "REDG", "MATCH", "LDG.E.128", "STG.E.128",
              "LDS.128", "STS.128", "SHFL", "MUFU"]
 
 

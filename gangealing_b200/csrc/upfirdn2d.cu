@@ -395,8 +395,9 @@ __device__ __forceinline__ void lane_strip(T* __restrict__ out_plane, const T* _
 // WARP-UNIFORM and, given the alignment S0 of the strip's first row and IW4 = in_w mod 4, a compile-time
 // constant per unrolled row: the kernel is instantiated per IW4 and branches once per task on S0, so the inner
 // loop is straight-line FMA code: no row/column tests, shuffles, selects or per-value address arithmetic.
-// Out-of-range columns are handled by folding a 0/1 mask into per-lane horizontal weights (the elements they
-// touch are real neighbours or zero-filled guards, hence finite).
+// Out-of-range columns are handled by folding a 0/1 mask into per-lane horizontal weights, so the elements they
+// touch must be finite: plan_band admits only pads whose stored outputs read columns -3 .. in_w + 2, i.e. real
+// neighbours in the flat slot or the 3 zero-filled elements in front of the first / behind the last virtual row.
 template <int IW4, int S0, bool FUSED, bool VEC>
 struct StripF32 {
   float* __restrict__ out_ptr;        // &out[plane][oys][x0]
@@ -718,6 +719,11 @@ struct BandPlan {
 inline bool plan_band(int dtype, int64_t planes, int in_h, int in_w, int out_h, int out_w, int pad_x0,
                       int pad_y0, const void* out, const void* noise, BandPlan* plan) {
   if (out_w < 24 || out_h < 8) return false;  // tiny planes: launch-bound, one thread per output is as good
+  // A stored output column ox reads input columns ox - pad_x0 .. ox - pad_x0 + 3 (zero taps included).  The fp32
+  // separable path weights out-of-range columns by zero instead of masking them, so each must be a real neighbour
+  // or one of the 3 zero-filled elements in front of / behind a slot's virtual rows: columns -3 .. in_w + 2.
+  // Wider pads (pad_x0 > 3, or pad_x1 + 4 - kernel_w > 3) go to the generic kernel.
+  if (pad_x0 > 3 || out_w - pad_x0 > in_w) return false;
   const int es = dtype_size(dtype);
   const int per16 = 16 / es;
   int lx_log2 = 5;

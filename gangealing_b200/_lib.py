@@ -144,7 +144,8 @@ def ptr(t):
 
 def is_nhwc(t):
     """True for a 4-D fp32 / bf16 tensor stored channels-last (and not also plain-contiguous).  The channels-last kernel
-    family moves 16 bytes of channels at a time: callers additionally check C % nhwc_vec(t) (or the blur's multiple)."""
+    family moves 16 bytes of channels at a time: op/nhwc.py's elementwise_ok / rowwise_ok / blur_ok add each kernel
+    family's channel limits."""
     return (t.dim() == 4 and t.dtype in (torch.float32, torch.bfloat16) and t.shape[1] > 1 and t.shape[2] * t.shape[3] > 1
             and t.is_contiguous(memory_format=torch.channels_last) and not t.is_contiguous())
 

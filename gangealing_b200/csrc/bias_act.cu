@@ -127,32 +127,51 @@ noise_bias_act_scalar_kernel(T* __restrict__ out, const T* __restrict__ x, const
   }
 }
 
-// Backward: gx = (out > 0 ? g : alpha*g) * scale, plus per-(row, chunk) partial sums of gx.
-// One CTA owns `chunk` consecutive elements of one (n,c) row (chunk == HW when HW is small and a CTA
-// then owns kRowsSmall... see launch code).  Partials are reduced by bias_grad_finish_kernel in a
-// fixed order -> bit-reproducible grad_bias (the reference's grad_input.sum() is not).
-template <typename T, int VEC>
+// Row-wise kernels over (rows, HW) planes, a row being one (n, c) plane, with one fp32 sum per row:
+//   MODE 0  channel scale       out = x*s[row]; with y, sum x*y   (modulating the INPUT of a weight-shared convolution,
+//                               networks.py:236/253 rewritten as conv(W, x*s); the sum is the gradient w.r.t. s)
+//   MODE 1  bias-act backward   out = (y > 0 ? x : alpha*x)*gain, y = the saved forward output; sum of out as stored,
+//                               as the reference's grad_input.sum() sums the stored gradient
+// Sums are finished by bias_grad_finish_kernel / row_finish_kernel in a fixed order -> bit-reproducible (the reference's
+// grad_input.sum() is not).
+template <typename T, int MODE>
+__device__ __forceinline__ void rowwise_op(float x, T y, bool has_y, float sv, float alpha, float gain, T& out,
+                                           float& acc) {
+  if constexpr (MODE == 0) {
+    out = Cvt<T>::from_f(x * sv);
+    if (has_y) acc = fmaf(x, Cvt<T>::to_f(y), acc);
+  } else {
+    const T r = Cvt<T>::from_f((Cvt<T>::to_f(y) > 0.f ? x : x * alpha) * gain);
+    out = r;
+    acc += Cvt<T>::to_f(r);
+  }
+}
+
+// One CTA owns `chunk` consecutive elements of one row and writes their sum to partial[blockIdx.x]
+// (blockIdx.x = row * chunks_per_row + chunk index).  VEC elements per access: 16 bytes (VEC = 16/sizeof(T)), or VEC = 1
+// scalar fallback.
+template <typename T, int VEC, int MODE>
 __global__ void __launch_bounds__(kThreads)
-bias_act_bwd_kernel(T* __restrict__ gx, float* __restrict__ partial, const T* __restrict__ g,
-                    const T* __restrict__ out, float alpha, float scale, int64_t HW, int64_t chunk,
-                    int chunks_per_row) {
-  // blockIdx.x = row * chunks_per_row + chunk_id
+rowwise_nchw_kernel(T* __restrict__ out, float* __restrict__ partial, const T* __restrict__ x, const T* __restrict__ y,
+                    const float* __restrict__ s, float alpha, float gain, int64_t HW, int64_t chunk, int chunks_per_row) {
   const int64_t row = blockIdx.x / chunks_per_row;
   const int ck = blockIdx.x - row * chunks_per_row;
   const int64_t p0 = static_cast<int64_t>(ck) * chunk;
   const int64_t p1 = min(p0 + chunk, HW);
   const int64_t off = row * HW;
+  const float sv = MODE == 0 ? __ldg(s + row) : 1.f;
+  const bool has_y = MODE == 1 || y != nullptr;
   float acc = 0.f;
   if constexpr (VEC > 1) {
     const int64_t nv = (p1 - p0) / VEC;  // chunk and HW are multiples of VEC on this path
     for (int64_t v0 = 0; v0 < nv; v0 += static_cast<int64_t>(kThreads) * kUnroll) {
-      Vec16<T> gv[kUnroll], ov[kUnroll];
+      Vec16<T> xv[kUnroll], yv[kUnroll];
 #pragma unroll
       for (int u = 0; u < kUnroll; ++u) {
         const int64_t v = v0 + u * kThreads + threadIdx.x;
         if (v < nv) {
-          gv[u] = ld_vec_stream(g + off + p0 + v * VEC);
-          ov[u] = ld_vec_stream(out + off + p0 + v * VEC);
+          xv[u] = ld_vec_stream(x + off + p0 + v * VEC);
+          if (has_y) yv[u] = ld_vec_stream(y + off + p0 + v * VEC);
         }
       }
 #pragma unroll
@@ -161,23 +180,16 @@ bias_act_bwd_kernel(T* __restrict__ gx, float* __restrict__ partial, const T* __
         if (v < nv) {
           Vec16<T> r;
 #pragma unroll
-          for (int k = 0; k < VEC; ++k) {
-            const float gg_ = Cvt<T>::to_f(gv[u].v[k]);
-            const float y = (Cvt<T>::to_f(ov[u].v[k]) > 0.f ? gg_ : gg_ * alpha) * scale;
-            r.v[k] = Cvt<T>::from_f(y);
-            acc += Cvt<T>::to_f(r.v[k]);  // sum what was stored (reference sums the stored grad_input)
-          }
-          st_vec_stream(gx + off + p0 + v * VEC, r);
+          for (int k = 0; k < VEC; ++k)
+            rowwise_op<T, MODE>(Cvt<T>::to_f(xv[u].v[k]), yv[u].v[k], has_y, sv, alpha, gain, r.v[k], acc);
+          st_vec_stream(out + off + p0 + v * VEC, r);
         }
       }
     }
   } else {
-    for (int64_t p = p0 + threadIdx.x; p < p1; p += kThreads) {
-      const float gg_ = Cvt<T>::to_f(g[off + p]);
-      const T y = Cvt<T>::from_f((Cvt<T>::to_f(out[off + p]) > 0.f ? gg_ : gg_ * alpha) * scale);
-      gx[off + p] = y;
-      acc += Cvt<T>::to_f(y);
-    }
+    for (int64_t p = p0 + threadIdx.x; p < p1; p += kThreads)
+      rowwise_op<T, MODE>(Cvt<T>::to_f(x[off + p]), has_y ? y[off + p] : T{}, has_y, sv, alpha, gain, out[off + p],
+                        acc);
   }
   if (partial) {
     __shared__ float wsum[kThreads / 32];
@@ -185,30 +197,30 @@ bias_act_bwd_kernel(T* __restrict__ gx, float* __restrict__ partial, const T* __
     if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = acc;
     __syncthreads();
     if (threadIdx.x == 0) {
-      float s = 0.f;
+      float t = 0.f;
 #pragma unroll
-      for (int w = 0; w < kThreads / 32; ++w) s += wsum[w];
-      partial[blockIdx.x] = s;
+      for (int w = 0; w < kThreads / 32; ++w) t += wsum[w];
+      partial[blockIdx.x] = t;
     }
   }
 }
 
-// Small-row variant: one warp per (n,c) row (HW < 1024), 8 rows per CTA.
-template <typename T>
+// Small rows (HW < 1024): one warp per row, 8 rows per CTA; the row's sum goes to partial[row].
+template <typename T, int MODE>
 __global__ void __launch_bounds__(kThreads)
-bias_act_bwd_rows_kernel(T* __restrict__ gx, float* __restrict__ partial, const T* __restrict__ g,
-                         const T* __restrict__ out, float alpha, float scale, int64_t rows, int64_t HW) {
+rowwise_nchw_rows_kernel(T* __restrict__ out, float* __restrict__ partial, const T* __restrict__ x,
+                         const T* __restrict__ y, const float* __restrict__ s, float alpha, float gain, int64_t rows,
+                         int64_t HW) {
   const int64_t row = static_cast<int64_t>(blockIdx.x) * (kThreads / 32) + (threadIdx.x >> 5);
   if (row >= rows) return;
   const int lane = threadIdx.x & 31;
   const int64_t off = row * HW;
+  const float sv = MODE == 0 ? __ldg(s + row) : 1.f;
+  const bool has_y = MODE == 1 || y != nullptr;
   float acc = 0.f;
-  for (int64_t p = lane; p < HW; p += 32) {
-    const float gg_ = Cvt<T>::to_f(g[off + p]);
-    const T y = Cvt<T>::from_f((Cvt<T>::to_f(out[off + p]) > 0.f ? gg_ : gg_ * alpha) * scale);
-    gx[off + p] = y;
-    acc += Cvt<T>::to_f(y);
-  }
+  for (int64_t p = lane; p < HW; p += 32)
+    rowwise_op<T, MODE>(Cvt<T>::to_f(x[off + p]), has_y ? y[off + p] : T{}, has_y, sv, alpha, gain, out[off + p],
+                        acc);
   if (partial) {
     acc = warp_sum(acc);
     if (lane == 0) partial[row] = acc;
@@ -230,89 +242,6 @@ __global__ void bias_grad_finish_kernel(float* __restrict__ grad_bias, const flo
   }
   acc = warp_sum(acc);
   if (lane == 0) grad_bias[c] = acc;
-}
-
-// out[n,c,p] = x[n,c,p] * s[n*C + c]   (modulating the INPUT of a weight-shared convolution, networks.py:236/253
-// rewritten as conv(W, x*s)); with `y` given, also row_dot[row] = sum_p x[row,p]*y[row,p] (the gradient w.r.t. s).
-template <typename T, int VEC>
-__global__ void __launch_bounds__(kThreads)
-channel_scale_kernel(T* __restrict__ out, float* __restrict__ partial, const T* __restrict__ x, const T* __restrict__ y,
-                     const float* __restrict__ s, int64_t HW, int64_t chunk, int chunks_per_row) {
-  const int64_t row = blockIdx.x / chunks_per_row;
-  const int ck = blockIdx.x - row * chunks_per_row;
-  const int64_t p0 = static_cast<int64_t>(ck) * chunk;
-  const int64_t p1 = min(p0 + chunk, HW);
-  const int64_t off = row * HW;
-  const float sv = __ldg(s + row);
-  float acc = 0.f;
-  if constexpr (VEC > 1) {
-    const int64_t nv = (p1 - p0) / VEC;
-    for (int64_t v0 = 0; v0 < nv; v0 += static_cast<int64_t>(kThreads) * kUnroll) {
-      Vec16<T> xv[kUnroll], yv[kUnroll];
-#pragma unroll
-      for (int u = 0; u < kUnroll; ++u) {
-        const int64_t v = v0 + u * kThreads + threadIdx.x;
-        if (v < nv) {
-          xv[u] = ld_vec_stream(x + off + p0 + v * VEC);
-          if (y) yv[u] = ld_vec_stream(y + off + p0 + v * VEC);
-        }
-      }
-#pragma unroll
-      for (int u = 0; u < kUnroll; ++u) {
-        const int64_t v = v0 + u * kThreads + threadIdx.x;
-        if (v < nv) {
-          Vec16<T> r;
-#pragma unroll
-          for (int k = 0; k < VEC; ++k) {
-            const float xf = Cvt<T>::to_f(xv[u].v[k]);
-            r.v[k] = Cvt<T>::from_f(xf * sv);
-            if (y) acc = fmaf(xf, Cvt<T>::to_f(yv[u].v[k]), acc);
-          }
-          st_vec_stream(out + off + p0 + v * VEC, r);
-        }
-      }
-    }
-  } else {
-    for (int64_t p = p0 + threadIdx.x; p < p1; p += kThreads) {
-      const float xf = Cvt<T>::to_f(x[off + p]);
-      out[off + p] = Cvt<T>::from_f(xf * sv);
-      if (y) acc = fmaf(xf, Cvt<T>::to_f(y[off + p]), acc);
-    }
-  }
-  if (partial) {
-    __shared__ float wsum[kThreads / 32];
-    acc = warp_sum(acc);
-    if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = acc;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      float t = 0.f;
-#pragma unroll
-      for (int w = 0; w < kThreads / 32; ++w) t += wsum[w];
-      partial[blockIdx.x] = t;
-    }
-  }
-}
-
-// small rows (HW < 1024): one warp per row, 8 rows per CTA
-template <typename T>
-__global__ void __launch_bounds__(kThreads)
-channel_scale_rows_kernel(T* __restrict__ out, float* __restrict__ row_dot, const T* __restrict__ x,
-                          const T* __restrict__ y, const float* __restrict__ s, int64_t rows, int64_t HW) {
-  const int64_t row = static_cast<int64_t>(blockIdx.x) * (kThreads / 32) + (threadIdx.x >> 5);
-  if (row >= rows) return;
-  const int lane = threadIdx.x & 31;
-  const int64_t off = row * HW;
-  const float sv = __ldg(s + row);
-  float acc = 0.f;
-  for (int64_t p = lane; p < HW; p += 32) {
-    const float xf = Cvt<T>::to_f(x[off + p]);
-    out[off + p] = Cvt<T>::from_f(xf * sv);
-    if (y) acc = fmaf(xf, Cvt<T>::to_f(y[off + p]), acc);
-  }
-  if (row_dot) {
-    acc = warp_sum(acc);
-    if (lane == 0) row_dot[row] = acc;
-  }
 }
 
 // row_dot[row] = sum_k partial[row*K + k]
@@ -383,58 +312,64 @@ int launch_noise(void* out, const void* x, const void* noise, const float* nw, c
   return GG_OK;
 }
 
-// geometry of the backward reduction, shared by the workspace query and the launch
-struct BwdGeom {
+// Geometry of the row-wise launch, shared by the workspace queries and the launch.  Each mode keeps its own chunk: a
+// different chunk regroups the partial sums, and so changes the bits of the reductions.
+struct RowGeom {
   bool small_rows;      // one warp per row
   int64_t chunk;        // elements per CTA within a row
-  int chunks_per_row;   // K
+  int chunks_per_row;   // K partial sums per row
 };
-inline BwdGeom bwd_geom(int64_t HW) {
-  BwdGeom g;
+inline RowGeom row_geom(int mode, int64_t HW) {
+  RowGeom g;
   g.small_rows = HW < 1024;
   if (g.small_rows) {
     g.chunk = HW;
     g.chunks_per_row = 1;
   } else {
-    g.chunk = 8192;  // 32 KB of fp32 per stream per CTA
+    g.chunk = mode == 0 ? 16384 : 8192;  // 64 KB / 32 KB of fp32 per stream per CTA
     g.chunks_per_row = static_cast<int>((HW + g.chunk - 1) / g.chunk);
   }
   return g;
 }
 
-template <typename T>
-int launch_bwd(void* gx, float* grad_bias, void* workspace, const void* g, const void* out, float alpha,
-               float scale, int64_t N, int64_t C, int64_t HW, cudaStream_t st) {
+// The row-wise kernel and its finishing reduction over N*C rows.  MODE 0: dst = row_dot[N*C] (gg_channel_scale passes
+// its rows as N, C = 1); MODE 1: dst = grad_bias[C].  `who` names the entry point in error messages.
+template <typename T, int MODE>
+int launch_rowwise(const char* who, void* out, float* dst, void* workspace, const void* x, const void* y, const float* s,
+                   float alpha, float gain, int64_t N, int64_t C, int64_t HW, cudaStream_t st) {
   constexpr int V = 16 / sizeof(T);
   const int64_t rows = N * C;
-  const BwdGeom geo = bwd_geom(HW);
-  float* partial = grad_bias ? static_cast<float*>(workspace) : nullptr;
+  const RowGeom geo = row_geom(MODE, HW);
+  // MODE 0's one-warp-per-row kernel writes row_dot itself; every other sum goes through the workspace
+  float* partial = !dst ? nullptr : (MODE == 0 && geo.small_rows) ? dst : static_cast<float*>(workspace);
+  auto* o = static_cast<T*>(out);
+  auto* xi = static_cast<const T*>(x);
+  auto* yi = static_cast<const T*>(y);
   if (geo.small_rows) {
     const int64_t grid = (rows + (kThreads / 32) - 1) / (kThreads / 32);
-    if (grid > 0x7fffffffLL) return fail(GG_ERR_BAD_ARG, "bias_act_backward: too many rows");
-    bias_act_bwd_rows_kernel<T><<<static_cast<unsigned>(grid), kThreads, 0, st>>>(
-        static_cast<T*>(gx), partial, static_cast<const T*>(g), static_cast<const T*>(out), alpha, scale,
-        rows, HW);
+    if (grid > 0x7fffffffLL) return fail(GG_ERR_BAD_ARG, "%s: too many rows", who);
+    rowwise_nchw_rows_kernel<T, MODE><<<static_cast<unsigned>(grid), kThreads, 0, st>>>(o, partial, xi, yi, s, alpha,
+                                                                                         gain, rows, HW);
   } else {
     const int64_t grid = rows * geo.chunks_per_row;
-    if (grid > 0x7fffffffLL) return fail(GG_ERR_BAD_ARG, "bias_act_backward: too many rows");
-    const bool vec = (HW % V == 0) && (geo.chunk % V == 0) && aligned16(gx) && aligned16(g) && aligned16(out);
+    if (grid > 0x7fffffffLL) return fail(GG_ERR_BAD_ARG, "%s: too many rows", who);
+    const bool vec = (HW % V == 0) && (geo.chunk % V == 0) && aligned16(out) && aligned16(x) && (!y || aligned16(y));
     if (vec)
-      bias_act_bwd_kernel<T, V><<<static_cast<unsigned>(grid), kThreads, 0, st>>>(
-          static_cast<T*>(gx), partial, static_cast<const T*>(g), static_cast<const T*>(out), alpha,
-          scale, HW, geo.chunk, geo.chunks_per_row);
+      rowwise_nchw_kernel<T, V, MODE><<<static_cast<unsigned>(grid), kThreads, 0, st>>>(
+          o, partial, xi, yi, s, alpha, gain, HW, geo.chunk, geo.chunks_per_row);
     else
-      bias_act_bwd_kernel<T, 1><<<static_cast<unsigned>(grid), kThreads, 0, st>>>(
-          static_cast<T*>(gx), partial, static_cast<const T*>(g), static_cast<const T*>(out), alpha,
-          scale, HW, geo.chunk, geo.chunks_per_row);
+      rowwise_nchw_kernel<T, 1, MODE><<<static_cast<unsigned>(grid), kThreads, 0, st>>>(
+          o, partial, xi, yi, s, alpha, gain, HW, geo.chunk, geo.chunks_per_row);
   }
-  GG_CHECK_LAUNCH("bias_act_backward launch");
-  if (grad_bias) {
+  GG_CHECK_LAUNCH("rowwise_nchw launch");
+  if (dst && MODE == 1) {
     const int warps = 4;
-    const int64_t grid = (C + warps - 1) / warps;
-    bias_grad_finish_kernel<<<static_cast<unsigned>(grid), warps * 32, 0, st>>>(grad_bias, partial, N, C,
-                                                                                geo.chunks_per_row);
+    bias_grad_finish_kernel<<<static_cast<unsigned>((C + warps - 1) / warps), warps * 32, 0, st>>>(dst, partial, N, C,
+                                                                                                  geo.chunks_per_row);
     GG_CHECK_LAUNCH("bias_grad_finish launch");
+  } else if (dst && !geo.small_rows) {
+    row_finish_kernel<<<static_cast<unsigned>((rows + 255) / 256), 256, 0, st>>>(dst, partial, rows, geo.chunks_per_row);
+    GG_CHECK_LAUNCH("row_finish launch");
   }
   return GG_OK;
 }
@@ -455,13 +390,10 @@ int gg_fused_bias_act(void* out, const void* x, const void* bias, const void* re
   if (act != 1 && act != 3) return fail(GG_ERR_UNSUPPORTED, "fused_bias_act: act must be 1 (linear) or 3 (lrelu)");
   if (grad < 0 || grad > 2) return fail(GG_ERR_BAD_ARG, "fused_bias_act: grad must be 0, 1 or 2");
   if (bias && (size_b <= 0 || step_b <= 0)) return fail(GG_ERR_BAD_ARG, "fused_bias_act: bias given with size_b/step_b <= 0");
-  auto st = static_cast<cudaStream_t>(stream);
-  switch (dtype) {
-    case GG_F32: return launch_flat<float>(out, x, bias, ref, act, grad, alpha, scale, size_x, step_b, size_b, st);
-    case GG_F16: return launch_flat<__half>(out, x, bias, ref, act, grad, alpha, scale, size_x, step_b, size_b, st);
-    case GG_BF16: return launch_flat<__nv_bfloat16>(out, x, bias, ref, act, grad, alpha, scale, size_x, step_b, size_b, st);
-    default: return fail(GG_ERR_UNSUPPORTED, "fused_bias_act: dtype %d not supported (f32/f16/bf16)", dtype);
-  }
+  GG_DISPATCH_T16(dtype, "fused_bias_act",
+                  return launch_flat<T_>(out, x, bias, ref, act, grad, alpha, scale, size_x, step_b, size_b,
+                                         static_cast<cudaStream_t>(stream)));
+  return GG_OK;
 }
 
 int gg_noise_bias_act(void* out, const void* x, const void* noise, const float* noise_weight,
@@ -470,19 +402,15 @@ int gg_noise_bias_act(void* out, const void* x, const void* noise, const float* 
   if (N < 0 || C < 0 || HW < 0) return fail(GG_ERR_BAD_ARG, "noise_bias_act: negative size");
   if (N * C * HW == 0) return GG_OK;
   if (!out || !x) return fail(GG_ERR_BAD_ARG, "noise_bias_act: null tensor");
-  auto st = static_cast<cudaStream_t>(stream);
-  switch (dtype) {
-    case GG_F32: return launch_noise<float>(out, x, noise, noise_weight, bias, row_scale, alpha, scale, N, C, HW, st);
-    case GG_F16: return launch_noise<__half>(out, x, noise, noise_weight, bias, row_scale, alpha, scale, N, C, HW, st);
-    case GG_BF16: return launch_noise<__nv_bfloat16>(out, x, noise, noise_weight, bias, row_scale, alpha, scale, N, C, HW, st);
-    default: return fail(GG_ERR_UNSUPPORTED, "noise_bias_act: dtype %d not supported", dtype);
-  }
+  GG_DISPATCH_T16(dtype, "noise_bias_act",
+                  return launch_noise<T_>(out, x, noise, noise_weight, bias, row_scale, alpha, scale, N, C, HW,
+                                          static_cast<cudaStream_t>(stream)));
+  return GG_OK;
 }
 
 int64_t gg_channel_scale_workspace(int64_t rows, int64_t HW) {
   if (rows <= 0 || HW <= 0) return 0;
-  const int64_t chunk = 16384;
-  return rows * ((HW + chunk - 1) / chunk) * static_cast<int64_t>(sizeof(float));
+  return rows * row_geom(0, HW).chunks_per_row * static_cast<int64_t>(sizeof(float));
 }
 
 int gg_channel_scale(void* out, float* row_dot, void* workspace, const void* x, const void* y, const float* s, int dtype,
@@ -491,53 +419,17 @@ int gg_channel_scale(void* out, float* row_dot, void* workspace, const void* x, 
   if (rows * HW == 0) return GG_OK;
   if (!out || !x || !s) return fail(GG_ERR_BAD_ARG, "channel_scale: null tensor");
   if (row_dot && (!y || !workspace)) return fail(GG_ERR_BAD_ARG, "channel_scale: row_dot needs y and a workspace");
-  const int64_t chunk = 16384;
-  const int K = static_cast<int>((HW + chunk - 1) / chunk);
-  const int64_t grid = rows * K;
-  if (grid > 0x7fffffffLL) return fail(GG_ERR_BAD_ARG, "channel_scale: too many rows");
-  auto st = static_cast<cudaStream_t>(stream);
-  float* partial = row_dot ? static_cast<float*>(workspace) : nullptr;
-  const void* yy = row_dot ? y : nullptr;
-  if (HW < 1024) {
-    const unsigned g = static_cast<unsigned>((rows + (kThreads / 32) - 1) / (kThreads / 32));
-    switch (dtype) {
-      case GG_F32: channel_scale_rows_kernel<float><<<g, kThreads, 0, st>>>(static_cast<float*>(out), row_dot, static_cast<const float*>(x), static_cast<const float*>(yy), s, rows, HW); break;
-      case GG_F16: channel_scale_rows_kernel<__half><<<g, kThreads, 0, st>>>(static_cast<__half*>(out), row_dot, static_cast<const __half*>(x), static_cast<const __half*>(yy), s, rows, HW); break;
-      case GG_BF16: channel_scale_rows_kernel<__nv_bfloat16><<<g, kThreads, 0, st>>>(static_cast<__nv_bfloat16*>(out), row_dot, static_cast<const __nv_bfloat16*>(x), static_cast<const __nv_bfloat16*>(yy), s, rows, HW); break;
-      default: return fail(GG_ERR_UNSUPPORTED, "channel_scale: dtype %d not supported", dtype);
-    }
-    GG_CHECK_LAUNCH("channel_scale_rows launch");
-    return GG_OK;
-  }
-#define GG_CS(T_)                                                                                                   \
-  do {                                                                                                              \
-    constexpr int V = 16 / sizeof(T_);                                                                              \
-    const bool vec = (HW % V == 0) && aligned16(out) && aligned16(x) && (!yy || aligned16(yy));                     \
-    if (vec)                                                                                                        \
-      channel_scale_kernel<T_, V><<<static_cast<unsigned>(grid), kThreads, 0, st>>>(                                \
-          static_cast<T_*>(out), partial, static_cast<const T_*>(x), static_cast<const T_*>(yy), s, HW, chunk, K);  \
-    else                                                                                                            \
-      channel_scale_kernel<T_, 1><<<static_cast<unsigned>(grid), kThreads, 0, st>>>(                                \
-          static_cast<T_*>(out), partial, static_cast<const T_*>(x), static_cast<const T_*>(yy), s, HW, chunk, K);  \
-  } while (0)
-  switch (dtype) {
-    case GG_F32: GG_CS(float); break;
-    case GG_F16: GG_CS(__half); break;
-    case GG_BF16: GG_CS(__nv_bfloat16); break;
-    default: return fail(GG_ERR_UNSUPPORTED, "channel_scale: dtype %d not supported", dtype);
-  }
-#undef GG_CS
-  GG_CHECK_LAUNCH("channel_scale launch");
-  if (row_dot) {
-    row_finish_kernel<<<static_cast<unsigned>((rows + 255) / 256), 256, 0, st>>>(row_dot, partial, rows, K);
-    GG_CHECK_LAUNCH("row_finish launch");
-  }
+  // this entry point's limit is rows x chunks, also for small rows where a CTA takes 8 rows (launch_rowwise counts CTAs)
+  if (rows * row_geom(0, HW).chunks_per_row > 0x7fffffffLL) return fail(GG_ERR_BAD_ARG, "channel_scale: too many rows");
+  GG_DISPATCH_T16(dtype, "channel_scale",
+                  return launch_rowwise<T_, 0>("channel_scale", out, row_dot, workspace, x, row_dot ? y : nullptr, s,
+                                               0.f, 1.f, rows, 1, HW, static_cast<cudaStream_t>(stream)));
   return GG_OK;
 }
 
 int64_t gg_bias_act_backward_workspace(int64_t N, int64_t C, int64_t HW) {
   if (N <= 0 || C <= 0 || HW <= 0) return 0;
-  return N * C * gg::bwd_geom(HW).chunks_per_row * static_cast<int64_t>(sizeof(float));
+  return N * C * row_geom(1, HW).chunks_per_row * static_cast<int64_t>(sizeof(float));
 }
 
 int gg_bias_act_backward(void* gx, float* grad_bias, void* workspace, const void* g, const void* out,
@@ -554,12 +446,10 @@ int gg_bias_act_backward(void* gx, float* grad_bias, void* workspace, const void
   }
   if (!gx || !g || !out) return fail(GG_ERR_BAD_ARG, "bias_act_backward: null tensor");
   if (grad_bias && !workspace) return fail(GG_ERR_BAD_ARG, "bias_act_backward: grad_bias needs a workspace");
-  switch (dtype) {
-    case GG_F32: return launch_bwd<float>(gx, grad_bias, workspace, g, out, alpha, scale, N, C, HW, st);
-    case GG_F16: return launch_bwd<__half>(gx, grad_bias, workspace, g, out, alpha, scale, N, C, HW, st);
-    case GG_BF16: return launch_bwd<__nv_bfloat16>(gx, grad_bias, workspace, g, out, alpha, scale, N, C, HW, st);
-    default: return fail(GG_ERR_UNSUPPORTED, "bias_act_backward: dtype %d not supported", dtype);
-  }
+  GG_DISPATCH_T16(dtype, "bias_act_backward",
+                  return launch_rowwise<T_, 1>("bias_act_backward", gx, grad_bias, workspace, g, out, nullptr, alpha,
+                                               scale, N, C, HW, st));
+  return GG_OK;
 }
 
 }  // extern "C"

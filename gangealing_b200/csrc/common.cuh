@@ -37,6 +37,25 @@ inline int cuda_fail(cudaError_t e, const char* what) {
     }                                                       \
   } while (0)
 
+// Storage-type dispatch: runs the statement(s) with T_ bound to the C type of `dtype_`; any other code returns
+// GG_ERR_UNSUPPORTED from the enclosing function.  GG_DISPATCH_T takes fp32 and bf16 (the channels-last kernels),
+// GG_DISPATCH_T16 fp16 as well.
+#define GG_DISPATCH_CASE_(code_, type_, ...) \
+  case code_: { using T_ = type_; __VA_ARGS__; break; }
+#define GG_DISPATCH_T(dtype_, who_, ...)                                                                             \
+  switch (dtype_) {                                                                                                  \
+    GG_DISPATCH_CASE_(GG_F32, float, __VA_ARGS__)                                                                    \
+    GG_DISPATCH_CASE_(GG_BF16, __nv_bfloat16, __VA_ARGS__)                                                           \
+    default: return ::gg::fail(GG_ERR_UNSUPPORTED, "%s: dtype %d not supported (fp32 or bf16)", who_, dtype_);       \
+  }
+#define GG_DISPATCH_T16(dtype_, who_, ...)                                                                           \
+  switch (dtype_) {                                                                                                  \
+    GG_DISPATCH_CASE_(GG_F32, float, __VA_ARGS__)                                                                    \
+    GG_DISPATCH_CASE_(GG_F16, __half, __VA_ARGS__)                                                                   \
+    GG_DISPATCH_CASE_(GG_BF16, __nv_bfloat16, __VA_ARGS__)                                                           \
+    default: return ::gg::fail(GG_ERR_UNSUPPORTED, "%s: dtype %d not supported (fp32, fp16 or bf16)", who_, dtype_); \
+  }
+
 int sm_count();  // defined in api.cu
 
 // One-time per-DEVICE configuration guard (cudaFuncSetAttribute is a per-device attribute, so a process that drives a

@@ -673,13 +673,6 @@ using namespace gg;
 
 extern "C" {
 
-#define GG_DISPATCH_T(dtype_, who_, ...)                                                                   \
-  switch (dtype_) {                                                                                        \
-    case GG_F32: { using T_ = float; __VA_ARGS__; break; }                                                 \
-    case GG_BF16: { using T_ = __nv_bfloat16; __VA_ARGS__; break; }                                        \
-    default: return fail(GG_ERR_UNSUPPORTED, "%s: dtype %d not supported (fp32 or bf16)", who_, dtype_);  \
-  }
-
 static inline int vec_of(int dtype) { return dtype == GG_BF16 ? 8 : 4; }
 
 int gg_noise_bias_act_nhwc(void* out, const void* x, const float* noise, const float* noise_weight, const float* bias,

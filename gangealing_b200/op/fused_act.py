@@ -10,14 +10,15 @@ from torch import nn
 from torch.autograd import Function
 
 from .. import _lib
+from . import nhwc
 
 
 def fused_bias_act_raw(x, bias, ref, act, grad, alpha, scale):
     """Python face of the reference's native `fused.fused_bias_act(input, bias, refer, act, grad, alpha,
     scale)` (fused_bias_act.cpp:11-17); `None`/empty tensors mean "no bias"/"no ref"."""
     _lib.require_cuda(x, bias, ref)
-    nhwc = _lib.is_nhwc(x) and (ref is None or (ref.shape == x.shape and ref.stride() == x.stride()))
-    if not nhwc:
+    cl = _lib.is_nhwc(x) and (ref is None or (ref.shape == x.shape and ref.stride() == x.stride()))
+    if not cl:
         x = x.contiguous()
     if bias is not None and bias.numel() == 0:
         bias = None
@@ -28,10 +29,10 @@ def fused_bias_act_raw(x, bias, ref, act, grad, alpha, scale):
     if ref is not None:
         if ref.shape != x.shape or ref.dtype != x.dtype:
             raise RuntimeError("fused_bias_act: ref must match the input's shape and dtype")
-        if not nhwc:
+        if not cl:
             ref = ref.contiguous()
     step_b = 1
-    if not nhwc:  # channels-last memory is (N*H*W, C): the bias index is simply i % C
+    if not cl:  # channels-last memory is (N*H*W, C): the bias index is simply i % C
         for s in x.shape[2:]:
             step_b *= s
     out = torch.empty_like(x)
@@ -45,9 +46,7 @@ def fused_bias_act_raw(x, bias, ref, act, grad, alpha, scale):
 def bias_act_backward_raw(grad_output, out, alpha, scale, want_bias_grad):
     """gx = (out > 0 ? g : alpha*g)*scale and, optionally, grad_bias = gx.sum(all dims but 1) (fp32)."""
     _lib.require_cuda(grad_output, out)
-    if (_lib.is_nhwc(out) and out.shape[1] % _lib.nhwc_vec(out) == 0 and out.shape[1] // _lib.nhwc_vec(out) <= 256
-            and grad_output.shape == out.shape):
-        from . import nhwc
+    if nhwc.rowwise_ok(out) and grad_output.shape == out.shape:
         g = grad_output.contiguous(memory_format=torch.channels_last)
         if g.dtype != out.dtype:
             g = g.to(out.dtype)
@@ -99,11 +98,9 @@ class FusedLeakyReLUFunction(Function):
     @staticmethod
     def forward(ctx, input, bias, negative_slope, scale):
         _lib.require_cuda(input, bias)
-        if (_lib.is_nhwc(input) and input.shape[1] % _lib.nhwc_vec(input) == 0
-                and (bias is None or bias.numel() in (0, input.shape[1]))):
+        if nhwc.elementwise_ok(input) and (bias is None or bias.numel() in (0, input.shape[1])):
             # channels-last: the 16-byte-vector streaming kernel of csrc/nhwc.cu (the flat kernel's per-element `i % C`
             # bias indexing is slower)
-            from . import nhwc
             b = bias if (bias is not None and bias.numel() > 0) else None
             out = nhwc.noise_bias_act(input, None, None, b, None, negative_slope, scale)
         else:

@@ -14,12 +14,12 @@ from torch.autograd import Function
 from torch.autograd.function import once_differentiable
 
 from .. import _lib
+from . import nhwc
 
 def channel_scale_raw(x, s, y=None):
     """out = x * s[n, c]; with `y`: also row_dot[n, c] = sum_hw x*y (fp32).  x: (N, C, H, W); s: (N, C) fp32."""
     _lib.require_cuda(x, s, y)
-    if _lib.is_nhwc(x) and x.shape[1] % _lib.nhwc_vec(x) == 0 and x.shape[1] // _lib.nhwc_vec(x) <= 256:
-        from . import nhwc
+    if nhwc.rowwise_ok(x):
         if y is not None:
             y = y.contiguous(memory_format=torch.channels_last)
             if y.dtype != x.dtype:

@@ -15,9 +15,22 @@ CL = torch.channels_last
 TIMING = None
 
 
-def blur_multiple(t):
-    """Channel multiple the TMA blur kernel wants: a CTA covers 8 threads x 16 bytes of channels."""
-    return 8 * _lib.nhwc_vec(t)
+# Which tensors each kernel family takes.  Every kernel moves 16 bytes of channels at a time (V = 4 fp32 / 8 bf16 channels).
+def elementwise_ok(t):
+    """noise_bias_act: a channels-last activation whose C is a multiple of V."""
+    return _lib.is_nhwc(t) and t.shape[1] % _lib.nhwc_vec(t) == 0
+
+
+def rowwise_ok(t):
+    """channel_scale, bias_act_backward: as elementwise, and C / V <= 256 (a CTA's threads cover one pixel's channels)."""
+    return elementwise_ok(t) and t.shape[1] // _lib.nhwc_vec(t) <= 256
+
+
+def blur_ok(t, kh, kw, up=(1, 1), down=(1, 1)):
+    """blur: C a multiple of 8 V (a CTA covers 8 threads x 16 bytes of channels), a filter of at most 4 x 4 taps and no
+    up- or down-sampling."""
+    return (_lib.is_nhwc(t) and t.shape[1] % (8 * _lib.nhwc_vec(t)) == 0 and kh <= 4 and kw <= 4
+            and up == (1, 1) and down == (1, 1))
 
 
 def _f32(t, numel=None):

@@ -10,22 +10,16 @@ import torch
 from torch.autograd import Function
 
 from .. import _lib
+from . import nhwc
 from .fused_act import bias_act_backward_raw
 from .modconv import channel_scale_raw
+from .nhwc import _f32
 from .upfirdn2d import UpFirDn2d, _taps, grad_pad
 
 
 # bench.py sets this to a list to time every fused-blur launch with CUDA events on the launching stream:
 # entries are (start_event, end_event, algorithmic_bytes).  None (default): no instrumentation.
 TIMING = None
-
-
-def _f32(t):
-    if t is None:
-        return None
-    if t.dtype != torch.float32 or not t.is_contiguous():
-        t = t.float().contiguous()
-    return t
 
 
 def _noise_plane(noise, x, out_h, out_w):
@@ -41,22 +35,20 @@ class _StyledTail(Function):
     @staticmethod
     def forward(ctx, x, noise, noise_weight, bias, kernel, pad, row_scale, negative_slope, scale):
         _lib.require_cuda(x, noise, noise_weight, bias, kernel, row_scale)
-        vec = _lib.nhwc_vec(x) if x.dtype in (torch.float32, torch.bfloat16) else 4
-        nhwc = _lib.is_nhwc(x) and x.shape[1] % (8 * vec if kernel is not None else vec) == 0
-        if not nhwc:
+        cl = nhwc.elementwise_ok(x) if kernel is None else nhwc.blur_ok(x, *kernel.shape)
+        if not cl:
             x = x.contiguous()
         n, c, in_h, in_w = x.shape
         lib = _lib.load()
         nw = _f32(noise_weight.reshape(-1)) if noise_weight is not None else None
         b = _f32(bias.reshape(-1)) if bias is not None else None
         rs = _f32(row_scale.reshape(-1)) if row_scale is not None else None
-        if nhwc:
-            from . import nhwc as K
+        if cl:
             if kernel is None:
-                out = K.noise_bias_act(x, noise, nw, b, rs, negative_slope, scale)
+                out = nhwc.noise_bias_act(x, noise, nw, b, rs, negative_slope, scale)
             else:
-                out = K.blur(x, kernel, pad, mode=1, noise=noise, noise_weight=nw, bias=b, row_scale=rs,
-                             negative_slope=negative_slope, gain=scale)[0]      # timed through op.nhwc.TIMING
+                out = nhwc.blur(x, kernel, pad, mode=1, noise=noise, noise_weight=nw, bias=b, row_scale=rs,
+                                negative_slope=negative_slope, gain=scale)[0]      # timed through op.nhwc.TIMING
         elif kernel is None:
             out = torch.empty_like(x)
             nz = _noise_plane(noise, x, in_h, in_w)

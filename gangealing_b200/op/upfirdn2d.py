@@ -9,6 +9,7 @@ import torch
 from torch.autograd import Function
 
 from .. import _lib
+from . import nhwc
 
 
 def _out_size(in_h, in_w, kh, kw, up, down, pad):
@@ -38,9 +39,8 @@ def upfirdn2d_raw(x, kernel, up, down, pad):
     out_h, out_w = _out_size(in_h, in_w, kh, kw, up, down, pad)
     if out_h < 1 or out_w < 1:
         raise RuntimeError("upfirdn2d: empty output (%d x %d)" % (out_h, out_w))
-    if (_lib.is_nhwc(x) and c % (8 * _lib.nhwc_vec(x)) == 0 and up == (1, 1) and down == (1, 1) and kh <= 4 and kw <= 4):
+    if nhwc.blur_ok(x, kh, kw, up, down):
         # channels-last activations stay channels-last (TMA tensor-map kernel, csrc/nhwc.cu; fp32 or bf16 storage)
-        from . import nhwc
         return nhwc.blur(x, kernel, pad, mode=0)[0]
     x = x.contiguous()
     out = torch.empty((n, c, out_h, out_w), dtype=x.dtype, device=x.device)

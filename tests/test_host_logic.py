@@ -50,6 +50,19 @@ def test_layout_predicate():
     assert _lib.is_nhwc(x.contiguous(memory_format=torch.channels_last))
     assert not _lib.is_nhwc(torch.zeros(2, 8, 1, 1).contiguous(memory_format=torch.channels_last))  # ambiguous: NCHW path
     assert not _lib.is_nhwc(torch.zeros(2, 8))
+    # which channels-last kernels take a tensor: 16-byte channel vectors (4 fp32 / 8 bf16), <= 256 of them per pixel for the
+    # row-wise kernels, 8 of them per CTA for the blur (<= 4x4 taps, no resampling)
+    from gangealing_b200.op import nhwc
+
+    def cl(c, dtype=torch.float32):
+        return torch.zeros(1, c, 2, 2, dtype=dtype).contiguous(memory_format=torch.channels_last)
+    assert nhwc.elementwise_ok(cl(4)) and not nhwc.elementwise_ok(cl(6)) and not nhwc.elementwise_ok(cl(4, torch.bfloat16))
+    assert not nhwc.elementwise_ok(cl(8, torch.float16)) and not nhwc.elementwise_ok(x)
+    assert nhwc.rowwise_ok(cl(1024)) and not nhwc.rowwise_ok(cl(1028)) and nhwc.elementwise_ok(cl(1028))
+    assert nhwc.rowwise_ok(cl(2048, torch.bfloat16)) and not nhwc.rowwise_ok(cl(2056, torch.bfloat16))
+    assert nhwc.blur_ok(cl(32), 4, 4) and not nhwc.blur_ok(cl(16), 4, 4) and not nhwc.blur_ok(cl(32, torch.bfloat16), 4, 4)
+    assert nhwc.blur_ok(cl(64, torch.bfloat16), 3, 4) and not nhwc.blur_ok(cl(32), 5, 4) and not nhwc.blur_ok(cl(32), 4, 5)
+    assert not nhwc.blur_ok(cl(32), 4, 4, (2, 2), (1, 1)) and not nhwc.blur_ok(cl(32), 4, 4, (1, 1), (1, 2))
 
 
 def test_upfirdn2d_size_arithmetic_matches_the_reference_formulae():

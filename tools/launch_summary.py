@@ -19,7 +19,7 @@ for r in rd:
     agg[short][1] += us
     total += us
 ours = ("fir4_band", "upfirdn2d_generic", "bias_act", "noise_bias_act", "bias_grad", "warp_", "mip_down", "flow_compose",
-        "splat_", "demod_umma", "modulate_kernel", "wsq_kernel", "blur_nhwc", "channel_scale", "rowwise_nhwc", "nhwc_finish",
+        "splat_", "demod_umma", "modulate_kernel", "wsq_kernel", "blur_nhwc", "channel_scale", "rowwise_", "nhwc_finish",
         "row_finish", "to_rgb_nhwc", "feature_distance", "distance_finish", "styled_tail", "tent_down", "fused_adam", "tv_loss",
         "nn_argmin", "lookup_splat", "warp_compose")
 def is_ours(k):   # every kernel of libgg_b200 lives in namespace gg (the name list is kept for pre-namespace captures)

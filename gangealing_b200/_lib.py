@@ -155,6 +155,19 @@ def nhwc_vec(t):
     return 8 if t.dtype == torch.bfloat16 else 4
 
 
+def aligned16(t):
+    """True when the tensor's data may be read 16 bytes at a time (a view with a storage offset may not)."""
+    return t.data_ptr() % 16 == 0
+
+
+def dense_f32(t):
+    """A contiguous fp32 tensor with 16-byte-aligned data: `t` itself when it already is one, else a copy.  The kernels
+    read per-channel constants as float4; a slice such as `b[1:]` is contiguous but 4 bytes off."""
+    if t.dtype != torch.float32 or not t.is_contiguous():
+        t = t.float().contiguous()
+    return t if aligned16(t) else t.clone()
+
+
 def tensor_cache(t):
     """Per-tensor-object memo, invalidated when the tensor is modified in place.  (Keyed on the Python object, not on
     data_ptr: a freed temporary's address can be handed to a different tensor.)"""

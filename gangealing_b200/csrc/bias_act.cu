@@ -253,8 +253,6 @@ __global__ void row_finish_kernel(float* __restrict__ row_dot, const float* __re
   row_dot[r] = acc;
 }
 
-inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
-
 template <typename T>
 int launch_flat(void* out, const void* x, const void* bias, const void* ref, int act, int grad,
                 float alpha, float scale, int64_t size_x, int64_t step_b, int64_t size_b,
@@ -416,7 +414,13 @@ int64_t gg_channel_scale_workspace(int64_t rows, int64_t HW) {
 int gg_channel_scale(void* out, float* row_dot, void* workspace, const void* x, const void* y, const float* s, int dtype,
                      int64_t rows, int64_t HW, void* stream) {
   if (rows < 0 || HW < 0) return fail(GG_ERR_BAD_ARG, "channel_scale: negative size");
-  if (rows * HW == 0) return GG_OK;
+  if (rows * HW == 0) {
+    if (row_dot && rows > 0) {   // the sum over an empty plane is 0
+      cudaError_t e = cudaMemsetAsync(row_dot, 0, rows * sizeof(float), static_cast<cudaStream_t>(stream));
+      if (e != cudaSuccess) return cuda_fail(e, "channel_scale memset");
+    }
+    return GG_OK;
+  }
   if (!out || !x || !s) return fail(GG_ERR_BAD_ARG, "channel_scale: null tensor");
   if (row_dot && (!y || !workspace)) return fail(GG_ERR_BAD_ARG, "channel_scale: row_dot needs y and a workspace");
   // this entry point's limit is rows x chunks, also for small rows where a CTA takes 8 rows (launch_rowwise counts CTAs)

@@ -58,6 +58,10 @@ inline int cuda_fail(cudaError_t e, const char* what) {
 
 int sm_count();  // defined in api.cu
 
+// True when `p` may be read as float4 / uint4.  Entry points whose kernels read a caller's pointer 16 bytes at a time
+// refuse a misaligned one (GG_ERR_BAD_ARG) before any launch; a null pointer passes.
+inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+
 // One-time per-DEVICE configuration guard (cudaFuncSetAttribute is a per-device attribute, so a process that drives a
 // second GPU must opt in there too).  Usage:  static DeviceOnce once;  if (once.needed()) { ...; once.done(); }
 struct DeviceOnce {

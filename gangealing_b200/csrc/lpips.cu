@@ -183,8 +183,9 @@ int launch_distance(float* partial, T* g0, T* g1, const float* gout, const T* f0
   return GG_OK;
 }
 
-int check_distance(const char* who, int64_t N, int C, int64_t HW) {
+int check_distance(const char* who, int64_t N, int C, int64_t HW, const float* weight) {
   if (N < 0 || C < 0 || HW < 0) return fail(GG_ERR_BAD_ARG, "%s: negative size", who);
+  if (!aligned16(weight)) return fail(GG_ERR_BAD_ARG, "%s: weight must be 16-byte aligned", who);   // read as float4
   if (C % 4 != 0 || C > 4 * 32 * kMaxTrips) return fail(GG_ERR_UNSUPPORTED, "%s: C must be a multiple of 4, <= 1024", who);
   const int c4 = C / 4;
   if (c4 < 32 && (c4 & (c4 - 1)) != 0) return fail(GG_ERR_UNSUPPORTED, "%s: C < 128 must be a power of two", who);
@@ -349,7 +350,7 @@ int64_t gg_feature_distance_workspace(int64_t N, int C, int64_t HW) {
 int gg_feature_distance_forward(float* out, void* workspace, const void* f0, const void* f1, const float* weight,
                                 int dtype, int64_t N, int C, int64_t HW, float eps, void* stream) {
   if (dtype != GG_F32 && dtype != GG_BF16) return fail(GG_ERR_UNSUPPORTED, "feature_distance: dtype %d not supported (fp32 or bf16)", dtype);
-  int rc = check_distance("feature_distance", N, C, HW);
+  int rc = check_distance("feature_distance", N, C, HW, weight);
   if (rc != GG_OK) return rc;
   if (N == 0) return GG_OK;
   if (!out) return fail(GG_ERR_BAD_ARG, "feature_distance: null output");
@@ -378,7 +379,7 @@ int gg_feature_distance_forward(float* out, void* workspace, const void* f0, con
 int gg_feature_distance_backward(void* g0, void* g1, const float* grad_out, const void* f0, const void* f1,
                                  const float* weight, int dtype, int64_t N, int C, int64_t HW, float eps, void* stream) {
   if (dtype != GG_F32 && dtype != GG_BF16) return fail(GG_ERR_UNSUPPORTED, "feature_distance backward: dtype %d not supported", dtype);
-  int rc = check_distance("feature_distance backward", N, C, HW);
+  int rc = check_distance("feature_distance backward", N, C, HW, weight);
   if (rc != GG_OK) return rc;
   if (N * HW == 0 || C == 0) return GG_OK;
   if (!grad_out || !f0 || !f1 || (!g0 && !g1)) return fail(GG_ERR_BAD_ARG, "feature_distance backward: null tensor");
@@ -402,6 +403,7 @@ int gg_bias_relu_pool_nhwc_forward(void* y, void* pooled, const void* raw, const
   const int64_t total = N * (H / 2) * static_cast<int64_t>(W / 2) * (C / V);
   if (total == 0) return GG_OK;
   if (!y || !pooled || !raw) return fail(GG_ERR_BAD_ARG, "bias_relu_pool: null tensor");
+  if (!aligned16(bias)) return fail(GG_ERR_BAD_ARG, "bias_relu_pool: bias must be 16-byte aligned");   // read as float4
   const int64_t grid = (total + 255) / 256;
   if (grid > 0x7fffffffLL) return fail(GG_ERR_BAD_ARG, "bias_relu_pool: tensor too large");
   auto st = static_cast<cudaStream_t>(stream);

@@ -685,6 +685,8 @@ int gg_noise_bias_act_nhwc(void* out, const void* x, const float* noise, const f
   const int V = vec_of(dtype);
   if (C % V != 0) return fail(GG_ERR_UNSUPPORTED, "noise_bias_act_nhwc: C must be a multiple of %d", V);
   if (!out || !x) return fail(GG_ERR_BAD_ARG, "noise_bias_act_nhwc: null tensor");
+  if (!aligned16(bias) || !aligned16(row_scale))   // read as float4
+    return fail(GG_ERR_BAD_ARG, "noise_bias_act_nhwc: bias and row_scale must be 16-byte aligned");
   const int64_t n_vec = numel / V;
   const int64_t grid = (n_vec + 4 * kT - 1) / (4 * kT);
   if (grid > 0x7fffffffLL) return fail(GG_ERR_BAD_ARG, "noise_bias_act_nhwc: tensor too large");
@@ -720,7 +722,15 @@ static int launch_rowwise(int mode, void* out, float* dst, void* workspace, cons
                           int dtype, float alpha, float gain, int64_t N, int C, int64_t HW, bool per_sample, void* stream) {
   if (N < 0 || C < 0 || HW < 0) return fail(GG_ERR_BAD_ARG, "nhwc rowwise: negative size");
   if (dtype != GG_F32 && dtype != GG_BF16) return fail(GG_ERR_UNSUPPORTED, "nhwc rowwise: dtype %d not supported", dtype);
-  if (N * HW * C == 0) return GG_OK;
+  if (N * HW * C == 0) {
+    // a sum over no pixels is 0: row_dot[N][C] (per sample) or grad_bias[C]
+    const int64_t sums = (per_sample ? N : 1) * C;
+    if (dst && sums > 0) {
+      cudaError_t e = cudaMemsetAsync(dst, 0, sums * sizeof(float), static_cast<cudaStream_t>(stream));
+      if (e != cudaSuccess) return cuda_fail(e, "nhwc rowwise memset");
+    }
+    return GG_OK;
+  }
   const int V = vec_of(dtype);
   if (C % V != 0 || C / V > kT) return fail(GG_ERR_UNSUPPORTED, "nhwc rowwise: C must be a multiple of %d and <= %d", V, V * kT);
   if (!out || !x) return fail(GG_ERR_BAD_ARG, "nhwc rowwise: null tensor");
@@ -778,6 +788,9 @@ int gg_to_rgb_nhwc_forward(float* out, const float* x, const float* wm, const fl
   if (N * HW == 0) return GG_OK;
   if (C < 32 || C % 32 != 0 || C > 1024) return fail(GG_ERR_UNSUPPORTED, "to_rgb_nhwc: C must be a multiple of 32, <= 1024");
   if (!out || !x || !wm) return fail(GG_ERR_BAD_ARG, "to_rgb_nhwc: null tensor");
+  // wm is read as float4; skip too, and out written as float4, when the planes are whole quads (HW % 4 == 0)
+  if (!aligned16(wm) || (HW % 4 == 0 && (!aligned16(skip) || !aligned16(out))))
+    return fail(GG_ERR_BAD_ARG, "to_rgb_nhwc: wm (and skip, out when HW %% 4 == 0) must be 16-byte aligned");
   // pixels per CTA: a multiple of the 128 pixels one trip covers, ~8 CTAs per SM over the whole batch
   const int64_t target = 8LL * sm_count();
   int64_t k = (target + N - 1) / N;
@@ -798,10 +811,17 @@ int gg_to_rgb_nhwc_forward(float* out, const float* x, const float* wm, const fl
 int gg_to_rgb_nhwc_backward(float* gx, float* gwm, void* workspace, const float* g, const float* x, const float* wm,
                             int64_t N, int C, int64_t HW, void* stream) {
   if (N < 0 || C < 0 || HW < 0) return fail(GG_ERR_BAD_ARG, "to_rgb_nhwc backward: negative size");
-  if (N * HW == 0 || C == 0) return GG_OK;
+  if (N * HW == 0 || C == 0) {
+    if (gwm && N * C > 0) {   // gwm sums over no pixels: 0
+      cudaError_t e = cudaMemsetAsync(gwm, 0, N * 3 * C * sizeof(float), static_cast<cudaStream_t>(stream));
+      if (e != cudaSuccess) return cuda_fail(e, "to_rgb_nhwc backward memset");
+    }
+    return GG_OK;
+  }
   if (C % 4 != 0 || C > 1024) return fail(GG_ERR_UNSUPPORTED, "to_rgb_nhwc backward: C must be a multiple of 4, <= 1024");
   if (!g || !wm || (!gx && !gwm)) return fail(GG_ERR_BAD_ARG, "to_rgb_nhwc backward: null tensor");
   if (gwm && (!x || !workspace)) return fail(GG_ERR_BAD_ARG, "to_rgb_nhwc backward: gwm needs x and a workspace");
+  if (!aligned16(wm)) return fail(GG_ERR_BAD_ARG, "to_rgb_nhwc backward: wm must be 16-byte aligned");   // read as float4
   const int c4 = C / 4;
   const int64_t chunk64 = rowwise_chunk(N, c4, HW);
   if (chunk64 > 0x7fffffffLL) return fail(GG_ERR_BAD_ARG, "to_rgb_nhwc backward: plane too large");

@@ -36,7 +36,7 @@ class _FeatureDistance(Function):
         _lib.require_cuda(f0, f1, weight)
         n, c, h, w = f0.shape
         lib = _lib.load()
-        wt = weight.detach().float().reshape(-1).contiguous() if weight is not None else None
+        wt = _lib.dense_f32(weight.detach().reshape(-1)) if weight is not None else None
         out = torch.empty(n, dtype=torch.float32, device=f0.device)
         ws = torch.empty(max(1, lib.gg_feature_distance_workspace(n, c, h * w) // 4), dtype=torch.float32, device=f0.device)
         rc = lib.gg_feature_distance_forward(out.data_ptr(), ws.data_ptr(), f0.data_ptr(), f1.data_ptr(), _lib.ptr(wt),
@@ -92,7 +92,7 @@ class _FeatureDistanceStacked(Function):
         n2, c, h, w = f.shape
         n = n2 // 2
         lib = _lib.load()
-        wt = weight.detach().float().reshape(-1).contiguous() if weight is not None else None
+        wt = _lib.dense_f32(weight.detach().reshape(-1)) if weight is not None else None
         out = torch.empty(n, dtype=torch.float32, device=f.device)
         ws = torch.empty(max(1, lib.gg_feature_distance_workspace(n, c, h * w) // 4), dtype=torch.float32, device=f.device)
         half = n * c * h * w * f.element_size()

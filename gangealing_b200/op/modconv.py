@@ -132,9 +132,9 @@ class _ToRGB(Function):
     def forward(ctx, x, wm, bias, skip):
         _lib.require_cuda(x, wm, bias, skip)
         n, c, h, w = x.shape
-        wmc = wm.detach().float().contiguous()
+        wmc = _lib.dense_f32(wm.detach())
         b = bias.detach().float().reshape(-1).contiguous() if bias is not None else None
-        sk = skip.detach().float().contiguous() if skip is not None else None
+        sk = _lib.dense_f32(skip.detach()) if skip is not None else None
         out = torch.empty((n, 3, h, w), dtype=torch.float32, device=x.device)
         rc = _lib.load().gg_to_rgb_nhwc_forward(out.data_ptr(), x.data_ptr(), wmc.data_ptr(), _lib.ptr(b), _lib.ptr(sk),
                                                 n, c, h * w, _lib.stream())
@@ -179,7 +179,7 @@ def modulated_conv2d(x, weight, style, scale, demodulate=True, upsample=False, p
         # to-RGB: a (3 x C) matrix per sample
         wm = (scale * weight[0, :, :, 0, 0]).unsqueeze(0) * style.unsqueeze(1)            # (B, O, I)
         b, _, h, w_ = x.shape
-        if _lib.is_nhwc(x) and o == 3 and i % 32 == 0 and i <= 1024 and x.dtype == torch.float32:
+        if _lib.is_nhwc(x) and o == 3 and i % 32 == 0 and i <= 1024 and x.dtype == torch.float32 and _lib.aligned16(x):
             return _ToRGB.apply(x, wm, bias, skip), None      # one fused pass over the channels-last activation
         if _lib.is_nhwc(x):   # (B, HW, I) @ (B, I, O): reads the channels-last activation in place
             rgb = torch.bmm(x.permute(0, 2, 3, 1).reshape(b, h * w_, i), wm.type(x.dtype).transpose(1, 2))

@@ -15,10 +15,11 @@ CL = torch.channels_last
 TIMING = None
 
 
-# Which tensors each kernel family takes.  Every kernel moves 16 bytes of channels at a time (V = 4 fp32 / 8 bf16 channels).
+# Which tensors each kernel family takes.  Every kernel moves 16 bytes of channels at a time (V = 4 fp32 / 8 bf16 channels),
+# so the activation must start on a 16-byte boundary (the blur's TMA descriptor needs that too).
 def elementwise_ok(t):
-    """noise_bias_act: a channels-last activation whose C is a multiple of V."""
-    return _lib.is_nhwc(t) and t.shape[1] % _lib.nhwc_vec(t) == 0
+    """noise_bias_act: a 16-byte-aligned channels-last activation whose C is a multiple of V."""
+    return _lib.is_nhwc(t) and t.shape[1] % _lib.nhwc_vec(t) == 0 and _lib.aligned16(t)
 
 
 def rowwise_ok(t):
@@ -30,15 +31,15 @@ def blur_ok(t, kh, kw, up=(1, 1), down=(1, 1)):
     """blur: C a multiple of 8 V (a CTA covers 8 threads x 16 bytes of channels), a filter of at most 4 x 4 taps and no
     up- or down-sampling."""
     return (_lib.is_nhwc(t) and t.shape[1] % (8 * _lib.nhwc_vec(t)) == 0 and kh <= 4 and kw <= 4
-            and up == (1, 1) and down == (1, 1))
+            and up == (1, 1) and down == (1, 1) and _lib.aligned16(t))
 
 
 def _f32(t, numel=None):
+    """`t` as dense, 16-byte-aligned fp32 (a copy when it is not).  Callers bind the result to a name until the launch: a
+    temporary freed while the argument list is still being built lets the next one reuse its memory."""
     if t is None:
         return None
-    t = t.detach()
-    if t.dtype != torch.float32 or not t.is_contiguous():
-        t = t.float().contiguous()
+    t = _lib.dense_f32(t.detach())
     if numel is not None and t.numel() != numel:
         raise RuntimeError("channels-last op: expected %d fp32 values, got %d" % (numel, t.numel()))
     return t
@@ -76,8 +77,10 @@ def blur(x, kernel, pad, mode=0, noise=None, noise_weight=None, bias=None, row_s
     nz = noise_plane(noise, n, out_h, out_w) if mode == 1 else None
     dot = ws = None
     if mode == 2 and want_dot:
-        if mul is None or mul.shape != (n, c, out_h, out_w) or mul.dtype != x.dtype or not mul.is_contiguous(memory_format=CL):
-            raise RuntimeError("blur (adjoint epilogue): `mul` must be a channels-last tensor of the output's shape and dtype")
+        if (mul is None or mul.shape != (n, c, out_h, out_w) or mul.dtype != x.dtype or not mul.is_contiguous(memory_format=CL)
+                or not _lib.aligned16(mul)):
+            raise RuntimeError("blur (adjoint epilogue): `mul` must be a 16-byte-aligned channels-last tensor of the output's "
+                               "shape and dtype")
         dot = torch.empty((n, c), dtype=torch.float32, device=x.device)
         nbytes = lib.gg_blur_nhwc_workspace(code, n, c, in_h, in_w, kh, kw, pad[0], pad[1], pad[2], pad[3])
         ws = torch.empty(max(1, nbytes // 4), dtype=torch.float32, device=x.device)
@@ -85,9 +88,10 @@ def blur(x, kernel, pad, mode=0, noise=None, noise_weight=None, bias=None, row_s
     if timed:
         ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         ev0.record()
+    nw, b, rs, s2 = _f32(noise_weight, 1), _f32(bias, c), _f32(row_scale, n * c), _f32(scale2, n * c)
     rc = lib.gg_blur_nhwc(_lib.ptr(out), _lib.ptr(out2), x.data_ptr(), taps.data_ptr(), _lib.ptr(nz),
-                          _lib.ptr(_f32(noise_weight, 1)), _lib.ptr(_f32(bias, c)), _lib.ptr(_f32(row_scale, n * c)),
-                          _lib.ptr(_f32(scale2, n * c)), _lib.ptr(mul if dot is not None else None), _lib.ptr(dot), _lib.ptr(ws),
+                          _lib.ptr(nw), _lib.ptr(b), _lib.ptr(rs),
+                          _lib.ptr(s2), _lib.ptr(mul if dot is not None else None), _lib.ptr(dot), _lib.ptr(ws),
                           code, n, c, in_h, in_w, kh, kw, 1 if _lib.filter_is_separable(kernel) else 0, pad[0], pad[1],
                           pad[2], pad[3], mode, act, negative_slope, gain, _lib.stream())
     _lib.check(rc, "gg_blur_nhwc")
@@ -103,10 +107,10 @@ def blur(x, kernel, pad, mode=0, noise=None, noise_weight=None, bias=None, row_s
 def noise_bias_act(x, noise, noise_weight, bias, row_scale, negative_slope, gain):
     n, c, h, w = x.shape
     out = torch.empty_like(x)
-    rc = _lib.load().gg_noise_bias_act_nhwc(out.data_ptr(), x.data_ptr(), _lib.ptr(noise_plane(noise, n, h, w)),
-                                            _lib.ptr(_f32(noise_weight, 1)), _lib.ptr(_f32(bias, c)),
-                                            _lib.ptr(_f32(row_scale, n * c)), _lib.dtype_code(x), negative_slope, gain,
-                                            n, c, h * w, _lib.stream())
+    nz, nw, b, rs = noise_plane(noise, n, h, w), _f32(noise_weight, 1), _f32(bias, c), _f32(row_scale, n * c)
+    rc = _lib.load().gg_noise_bias_act_nhwc(out.data_ptr(), x.data_ptr(), _lib.ptr(nz), _lib.ptr(nw), _lib.ptr(b),
+                                            _lib.ptr(rs), _lib.dtype_code(x), negative_slope, gain, n, c, h * w,
+                                            _lib.stream())
     _lib.check(rc, "gg_noise_bias_act_nhwc")
     return out
 
@@ -133,7 +137,8 @@ def channel_scale(x, s, y=None):
     if y is not None:
         dot = torch.empty((n, c), dtype=torch.float32, device=x.device)
         ws = torch.empty(max(1, lib.gg_nhwc_rowwise_workspace(n, c, h * w) // 4), dtype=torch.float32, device=x.device)
-    rc = lib.gg_channel_scale_nhwc(out.data_ptr(), _lib.ptr(dot), _lib.ptr(ws), x.data_ptr(), _lib.ptr(y), _f32(s, n * c).data_ptr(),
+    sc = _f32(s, n * c)
+    rc = lib.gg_channel_scale_nhwc(out.data_ptr(), _lib.ptr(dot), _lib.ptr(ws), x.data_ptr(), _lib.ptr(y), sc.data_ptr(),
                                    _lib.dtype_code(x), n, c, h * w, _lib.stream())
     _lib.check(rc, "gg_channel_scale_nhwc")
     return out, dot
@@ -152,10 +157,10 @@ def styled_tail(raw, noise, noise_weight, bias, demod, s_next, wm, rgb_bias, ski
             sk = sk.float().contiguous()
         if sk.shape != rgb.shape:
             raise RuntimeError("styled_tail: skip must be (N, 3, H, W)")
+    consts = [noise_plane(noise, n, h, w), _f32(noise_weight, 1), _f32(bias, c), _f32(demod, n * c), _f32(s_next, n * c),
+              _f32(wm, n * 3 * c), _f32(rgb_bias, 3)]
     rc = _lib.load().gg_styled_tail_nhwc(_lib.ptr(out), _lib.ptr(xs), _lib.ptr(rgb), raw.data_ptr(),
-                                         _lib.ptr(noise_plane(noise, n, h, w)), _lib.ptr(_f32(noise_weight, 1)),
-                                         _lib.ptr(_f32(bias, c)), _lib.ptr(_f32(demod, n * c)), _lib.ptr(_f32(s_next, n * c)),
-                                         _lib.ptr(_f32(wm, n * 3 * c)), _lib.ptr(_f32(rgb_bias, 3)), _lib.ptr(sk),
+                                         *[_lib.ptr(t) for t in consts], _lib.ptr(sk),
                                          _lib.dtype_code(raw), act, negative_slope, gain, n, c, h * w, _lib.stream())
     _lib.check(rc, "gg_styled_tail_nhwc")
     return out, xs, rgb
@@ -185,10 +190,11 @@ def styled_tail_backward(g_xs, g_rgb, out_saved, raw, s_next, demod, wm, want_ds
     ws = None
     if rows:
         ws = torch.empty(max(1, lib.gg_styled_tail_backward_workspace(code, n, c, h * w) // 4), dtype=torch.float32, device=dev)
+    consts = [_f32(s_next, n * c), _f32(demod, n * c), _f32(wm, n * 3 * c)]
     rc = lib.gg_styled_tail_backward_nhwc(g_raw.data_ptr(), _lib.ptr(d_s), _lib.ptr(d_d), _lib.ptr(d_w), _lib.ptr(ws),
                                           _lib.ptr(g_xs), _lib.ptr(g_rgb), out_saved.data_ptr(),
                                           _lib.ptr(raw if want_dd else None),
-                                          _lib.ptr(_f32(s_next, n * c)), _lib.ptr(_f32(demod, n * c)), _lib.ptr(_f32(wm, n * 3 * c)),
+                                          *[_lib.ptr(t) for t in consts],
                                           code, negative_slope, gain, n, c, h * w, rows * c, _lib.stream())
     _lib.check(rc, "gg_styled_tail_backward_nhwc")
     return g_raw, d_s, d_d, d_w

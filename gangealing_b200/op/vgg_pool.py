@@ -27,7 +27,7 @@ class _BiasReluPool(Function):
         n, c, h, w = raw.shape
         y = torch.empty_like(raw)                                       # channels-last like raw
         pooled = torch.empty(n, c, h // 2, w // 2, dtype=raw.dtype, device=raw.device, memory_format=torch.channels_last)
-        b = None if bias is None else bias.detach().float().contiguous()
+        b = None if bias is None else _lib.dense_f32(bias.detach())
         with torch.cuda.device(raw.device):
             _lib.check(_lib.load().gg_bias_relu_pool_nhwc_forward(y.data_ptr(), pooled.data_ptr(), raw.data_ptr(), _lib.ptr(b),
                                                                   _lib.dtype_code(raw), n, c, h, w, _lib.stream()),

@@ -94,3 +94,23 @@ def test_argument_validation_of_the_channels_last_and_loss_entry_points():
     assert dll.gg_styled_tail_backward_nhwc(one, None, None, None, None, one, None, one, None, None, None, None,
                                             0, 0.2, 1.0, 1, 32, 16, 32, None) == -1                      # g_xs without s_next
     assert dll.gg_styled_tail_backward_workspace(0, 2, 64, 256) > 0
+
+
+def test_misaligned_vector_operands_are_refused():
+    """Kernels that read a per-channel constant as float4 refuse a pointer off a 16-byte boundary (a slice such as b[1:])
+    with a status code, before any device work, instead of faulting on the device."""
+    dll = _lib.load()
+    a, m = 16, 4     # an aligned and a misaligned non-null pointer value; validation must not dereference either
+
+    def refused(rc):
+        return rc == -1 and b"aligned" in dll.gg_last_error()
+    assert refused(dll.gg_noise_bias_act_nhwc(a, a, None, None, m, None, 0, 0.2, 1.0, 1, 8, 16, None))          # bias
+    assert refused(dll.gg_noise_bias_act_nhwc(a, a, None, None, None, m, 2, 0.2, 1.0, 1, 8, 16, None))          # row_scale
+    assert refused(dll.gg_to_rgb_nhwc_forward(a, a, m, None, None, 1, 32, 16, None))                            # wm
+    assert refused(dll.gg_to_rgb_nhwc_forward(a, a, a, None, m, 1, 32, 16, None))                               # skip, HW % 4 == 0
+    assert refused(dll.gg_to_rgb_nhwc_backward(a, None, None, a, a, m, 1, 32, 16, None))                        # wm
+    assert refused(dll.gg_bias_relu_pool_nhwc_forward(a, a, a, m, 0, 1, 8, 4, 4, None))                         # bias
+    assert refused(dll.gg_feature_distance_forward(a, a, a, a, m, 0, 2, 64, 16, 1e-10, None))                   # weight
+    assert refused(dll.gg_feature_distance_backward(a, a, a, a, a, m, 2, 2, 64, 16, 1e-10, None))               # weight
+    # the shape contracts are still checked first
+    assert dll.gg_to_rgb_nhwc_forward(a, a, m, None, None, 1, 20, 16, None) == -2

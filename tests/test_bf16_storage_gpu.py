@@ -89,17 +89,19 @@ def finish_depth(k):
     return _ceil(k, 32) + 2 + 32
 
 
-def rowwise_geometry(n, cv, hw):
-    """rowwise_chunk / bwd_chunk of csrc/nhwc.cu, csrc/styled.cu: (pixel lanes, pixels per CTA, CTAs per sample)."""
+def rowwise_geometry(n, cv, hw, sms=None):
+    """rowwise_chunk / bwd_chunk of csrc/nhwc.cu, csrc/styled.cu for C/V = cv channel vectors, planned for `sms` SMs (default:
+    this device's): (pixel lanes, pixels per CTA, CTAs per sample)."""
     lanes = max(256 // cv, 1)
-    k = max(1, min(_ceil(8 * _sm(), n), _ceil(hw, 4 * lanes)))
+    k = max(1, min(_ceil(8 * (sms or _sm()), n), _ceil(hw, 4 * lanes)))
     chunk = _ceil(hw, k)
     return lanes, chunk, _ceil(hw, chunk)
 
 
-def rowwise_c(n, c, hw, per_term, per_sample):
-    """A thread's serial sum over its pixels, the CTA's pixel lanes in order, then the finish kernel over the CTAs."""
-    lanes, chunk, k = rowwise_geometry(n, c // 8, hw)
+def rowwise_c(n, c, hw, per_term, per_sample, v=8, sms=None):
+    """A thread's serial sum over its pixels, the CTA's pixel lanes in order, then the finish kernel over the CTAs.
+    v: channels per 16-byte vector (8 bf16, 4 fp32)."""
+    lanes, chunk, k = rowwise_geometry(n, c // v, hw, sms)
     return per_term + _ceil(chunk, lanes) + lanes + finish_depth(k if per_sample else n * k)
 
 

@@ -63,6 +63,27 @@ def test_layout_predicate():
     assert nhwc.blur_ok(cl(32), 4, 4) and not nhwc.blur_ok(cl(16), 4, 4) and not nhwc.blur_ok(cl(32, torch.bfloat16), 4, 4)
     assert nhwc.blur_ok(cl(64, torch.bfloat16), 3, 4) and not nhwc.blur_ok(cl(32), 5, 4) and not nhwc.blur_ok(cl(32), 4, 5)
     assert not nhwc.blur_ok(cl(32), 4, 4, (2, 2), (1, 1)) and not nhwc.blur_ok(cl(32), 4, 4, (1, 1), (1, 2))
+    # the activation itself is read 16 bytes at a time: a view one element past a 16-byte boundary takes the NCHW route,
+    # one a whole 16 bytes past keeps the channels-last one
+    def at(c, off, dtype=torch.float32):
+        buf = torch.zeros(off + 4 * c, dtype=dtype)
+        return buf[off:].as_strided((1, c, 2, 2), (4 * c, 1, 2 * c, c))
+    for c, dtype in ((32, torch.float32), (64, torch.bfloat16)):
+        step = 16 // torch.tensor([], dtype=dtype).element_size()
+        aligned = at(c, 0, dtype)
+        assert aligned.data_ptr() % 16 == 0 and _lib.is_nhwc(aligned)
+        assert nhwc.elementwise_ok(aligned) and nhwc.rowwise_ok(aligned) and nhwc.blur_ok(aligned, 4, 4)
+        assert nhwc.elementwise_ok(at(c, step, dtype)) and nhwc.blur_ok(at(c, step, dtype), 4, 4)
+        off = at(c, 1, dtype)
+        assert _lib.is_nhwc(off) and off.data_ptr() % 16 != 0
+        assert not nhwc.elementwise_ok(off) and not nhwc.rowwise_ok(off) and not nhwc.blur_ok(off, 4, 4)
+    # per-channel constants reach the kernels as 16-byte-aligned fp32: a slice is copied, a whole tensor is not
+    b = torch.arange(9, dtype=torch.float32)
+    assert nhwc._f32(b) is not None and nhwc._f32(b).data_ptr() == b.data_ptr()
+    s = nhwc._f32(b[1:], 8)
+    assert s.data_ptr() % 16 == 0 and s.data_ptr() != b[1:].data_ptr() and torch.equal(s, b[1:])
+    assert _lib.dense_f32(b[4:]).data_ptr() == b[4:].data_ptr()
+    assert _lib.dense_f32(b[1:].double()).dtype == torch.float32
 
 
 def test_upfirdn2d_size_arithmetic_matches_the_reference_formulae():

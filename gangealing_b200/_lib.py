@@ -38,6 +38,9 @@ SIGNATURES = {
     "gg_mipmap_warp_forward": (_I, [_P] * 5 + [_I, _L] + [_I] * 6 + [_F, _F, _I, _P]),
     "gg_warp_sample_indices": (_I, [_P, _P, _L, _I, _I, _I, _I, _F, _F, _I, _P]),
     "gg_stn_sample_forward": (_I, [_P] * 11 + [_I, _I, _L] + [_I] * 9 + [_F, _F, _I, _P]),
+    "gg_mipmap_warp_lerp_forward": (_I, [_P] * 5 + [_L, _P, _P, _I, _I, _L] + [_I] * 6 + [_F, _F, _I, _P]),
+    "gg_mipmap_warp_lerp_mean": (_I, [_P] * 4 + [_L, _P, _P, _I, _I, _L] + [_I] * 6 + [_F, _F, _I, _I, _P]),
+    "gg_track_points_lerp": (_I, [_P] * 6 + [_I, _L, _L, _I, _I, _I, _P]),
     "gg_modconv_wsq": (_I, [_P, _P, _I, _I, _I, _P]),
     "gg_modconv_demod": (_I, [_P, _P, _P, _F, _F, _I, _I, _I, _P]),
     "gg_modconv_demod_batched": (_I, [_I, _P, _P, _P, _P, _P, _P, _F, _I, _P]),

@@ -337,23 +337,45 @@ sample_indices_kernel(int4* __restrict__ out, const float* __restrict__ grid, co
 // and then runs the level-of-detail / trilinear sampling.  The generated grid (and the residual flow the TV regulariser
 // needs) are WRITTEN as by-products (the callers return them), replacing affine_grid (a bmm + 3 elementwise launches) or the
 // separate flow_compose pass and the grid read-back.
+//   MODE 3 (vis_correspondence.py:183-205, :335-380): a lerp of two grids, g = lerp(base[n], target[n], alphas[t]), for T
+//           lerp weights at once (one CTA row per (frame, sample); the pyramid serves every frame)
 struct ComposeParams {
   const float* grid;      // MODE 0: (N, Ho, Wo, 2) sampling grid
   const float* theta;     // MODE 1: (N, 2, 3) sampling matrices.  MODE 2: base warp (N, 2, 3) or null
   const float* low;       // MODE 2: (N, lh, lw, 2)
   const float* mask;      // MODE 2: (N, 9*s*s, lh, lw)
   const float* identity;  // MODE 2: (s*lh, s*lw, 2) identity sampling grid (the head's buffer)
-  const float* alpha;     // MODE 2: (N) or null
+  const float* alpha;     // MODE 2: (N) or null.  MODE 3: (T) lerp weights
   int lh, lw, s;
-  float* grid_out;        // MODES 1, 2: (N, Ho, Wo, 2) or null
+  float* grid_out;        // MODES 1, 2: (N, Ho, Wo, 2) or null.  MODE 3: (T, N, Ho, Wo, 2) or null
   float* delta_out;       // MODE 2: (N, Ho, Wo, 2) or null
+  const float* base;      // MODE 3: (N or 1, Ho, Wo, 2), sample stride base_stride floats (0: one broadcast grid)
+  const float* target;    // MODE 3: (N, Ho, Wo, 2)
+  int64_t base_stride;
+  int frames;             // MODE 3: T
 };
+
+// torch.lerp (ATen/native/Lerp.h: |w| < 0.5 ? a + w (b - a) : b - (b - a)(1 - w)), with the contractions nvcc makes in
+// ATen's lerp kernel, so that a lerped grid is bitwise torch.lerp's on the device
+__device__ __forceinline__ float lerp_aten(float a, float b, float w) {
+  const float d = b - a;
+  return (fabsf(w) < 0.5f) ? fmaf(w, d, a) : fmaf(-d, 1.f - w, b);
+}
+
+__device__ __forceinline__ float2 lerp_aten(float2 a, float2 b, float w) {
+  return make_float2(lerp_aten(a.x, b.x, w), lerp_aten(a.y, b.y, w));
+}
 
 template <int MODE>
 __device__ __forceinline__ float2 compose_at(const ComposeParams& cp, const WarpParams& p, int64_t n, int y, int x,
-                                             float2* delta) {
+                                             float2* delta, float w = 0.f) {
   if (MODE == 0) {
     return __ldg(reinterpret_cast<const float2*>(cp.grid + ((n * p.ho + y) * static_cast<int64_t>(p.wo) + x) * 2));
+  } else if (MODE == 3) {
+    const int64_t pix = (static_cast<int64_t>(y) * p.wo + x) * 2;
+    const float2 a = __ldg(reinterpret_cast<const float2*>(cp.base + n * cp.base_stride + pix));
+    const float2 b = __ldg(reinterpret_cast<const float2*>(cp.target + n * p.ho * static_cast<int64_t>(p.wo) * 2 + pix));
+    return lerp_aten(a, b, w);
   } else if (MODE == 1) {
     const float* M = cp.theta + n * 6;
     const float bx = (2.f * static_cast<float>(x) + 1.f) / static_cast<float>(p.wo) - 1.f;
@@ -373,6 +395,30 @@ __device__ __forceinline__ float2 compose_at(const ComposeParams& cp, const Warp
 // and parks it in shared memory together with the one-pixel halo (by the first 84 threads), so the level of detail reads its
 // 4 neighbours from shared memory instead of regenerating them (5x fewer softmax evaluations than a per-thread recompute).
 constexpr int kTileX = 32, kTileY = 8;
+constexpr int kRing = 2 * (kTileX + 2) + 2 * kTileY;   // halo positions around a tile
+
+// Halo position (hy, hx) in tile coordinates (-1 .. kTile) of ring slot r < kRing.
+__device__ __forceinline__ void halo_slot(int r, int& hy, int& hx) {
+  if (r < kTileX + 2) { hy = -1; hx = r - 1; }
+  else if (r < 2 * (kTileX + 2)) { hy = kTileY; hx = r - (kTileX + 2) - 1; }
+  else if (r < 2 * (kTileX + 2) + kTileY) { hy = r - 2 * (kTileX + 2); hx = -1; }
+  else { hy = r - 2 * (kTileX + 2) - kTileY; hx = kTileX; }
+}
+
+// Output value of one channel plane at a pixel whose corners `s` and levels (l0, l1, w) are known: the bilinear sample of
+// level l0, blended with level l1.  Both forward kernels call this, so a frame mean adds the per-sample kernel's values.
+template <typename T, bool MIP>
+__device__ __forceinline__ float sample_channel(const T* __restrict__ src, const float* __restrict__ pyr, const WarpParams& p,
+                                                int64_t plane, int l0, int l1, float w, const SampleGeom& s) {
+  const T* src_plane = src + plane * p.hs * static_cast<int64_t>(p.ws);
+  const float o0 = sample_level<T, false>(src_plane, pyr, p, plane, l0, s, nullptr, nullptr);
+  float o = o0;
+  if (MIP && l1 != l0) {
+    const float o1 = sample_level<T, false>(src_plane, pyr, p, plane, l1, s, nullptr, nullptr);
+    o = o0 + w * (o1 - o0);
+  }
+  return o;
+}
 
 template <typename T, bool MIP, int MODE>
 __global__ void __launch_bounds__(kTileX * kTileY)
@@ -382,36 +428,33 @@ warp_compose_fwd_kernel(T* __restrict__ out, float* __restrict__ levels_out, con
   __shared__ float2 tile[kTileY + 2][kTileX + 2];
   const int tx = threadIdx.x % kTileX, ty = threadIdx.x / kTileX;
   const int bx = blockIdx.x % tiles_x, by = (blockIdx.x / tiles_x) % tiles_y;
-  const int64_t n = blockIdx.x / (tiles_x * tiles_y);
+  const int64_t tn = blockIdx.x / (tiles_x * tiles_y);   // output image: MODE 3 frame * N + sample, else the sample
+  const int64_t n = (MODE == 3) ? tn % p.n : tn;         // source sample
+  const float lw = (MODE == 3) ? __ldg(cp.alpha + tn / p.n) : 0.f;
   const int x0 = bx * kTileX, y0 = by * kTileY;
   const int ox = x0 + tx, oy = y0 + ty;
   const bool live = ox < p.wo && oy < p.ho;
   float2 delta = make_float2(0.f, 0.f);
   float2 g = make_float2(0.f, 0.f);
   if (live) {
-    g = compose_at<MODE>(cp, p, n, oy, ox, &delta);
-    const int64_t idx = (n * p.ho + oy) * static_cast<int64_t>(p.wo) + ox;
+    g = compose_at<MODE>(cp, p, n, oy, ox, &delta, lw);
+    const int64_t idx = (tn * p.ho + oy) * static_cast<int64_t>(p.wo) + ox;
     if (cp.grid_out) *reinterpret_cast<float2*>(cp.grid_out + idx * 2) = g;
     if (MODE == 2 && cp.delta_out) *reinterpret_cast<float2*>(cp.delta_out + idx * 2) = delta;
   }
   tile[ty + 1][tx + 1] = g;
   if (MIP) {
     // halo ring: 2*(kTileX + 2) + 2*kTileY = 84 positions, replicate-clamped to the image like the reference's neighbours
-    constexpr int kRing = 2 * (kTileX + 2) + 2 * kTileY;
     if (threadIdx.x < kRing) {
       int hy, hx;
-      const int r = threadIdx.x;
-      if (r < kTileX + 2) { hy = -1; hx = r - 1; }
-      else if (r < 2 * (kTileX + 2)) { hy = kTileY; hx = r - (kTileX + 2) - 1; }
-      else if (r < 2 * (kTileX + 2) + kTileY) { hy = r - 2 * (kTileX + 2); hx = -1; }
-      else { hy = r - 2 * (kTileX + 2) - kTileY; hx = kTileX; }
+      halo_slot(threadIdx.x, hy, hx);
       const int yy = min(max(y0 + hy, 0), p.ho - 1), xx = min(max(x0 + hx, 0), p.wo - 1);
-      tile[hy + 1][hx + 1] = compose_at<MODE>(cp, p, n, yy, xx, nullptr);
+      tile[hy + 1][hx + 1] = compose_at<MODE>(cp, p, n, yy, xx, nullptr, lw);
     }
     __syncthreads();
   }
   if (!live) return;
-  const int64_t idx = (n * p.ho + oy) * static_cast<int64_t>(p.wo) + ox;
+  const int64_t idx = (tn * p.ho + oy) * static_cast<int64_t>(p.wo) + ox;
   const SampleGeom s = sample_geom(g.x, g.y, p.hs, p.ws, p.pad_mode);
   int l0 = 0, l1 = 0;
   float w = 0.f;
@@ -425,15 +468,85 @@ warp_compose_fwd_kernel(T* __restrict__ out, float* __restrict__ levels_out, con
     if (levels_out) levels_out[idx] = li.level;
   }
   for (int c = 0; c < p.c; ++c) {
-    const int64_t plane = n * p.c + c;
-    const T* src_plane = src + plane * p.hs * static_cast<int64_t>(p.ws);
-    const float o0 = sample_level<T, false>(src_plane, pyr, p, plane, l0, s, nullptr, nullptr);
-    float o = o0;
-    if (MIP && l1 != l0) {
-      const float o1 = sample_level<T, false>(src_plane, pyr, p, plane, l1, s, nullptr, nullptr);
-      o = o0 + w * (o1 - o0);
+    const float o = sample_channel<T, MIP>(src, pyr, p, n * p.c + c, l0, l1, w, s);
+    out[((tn * p.c + c) * p.ho + oy) * static_cast<int64_t>(p.wo) + ox] = Cvt<T>::from_f(o);
+  }
+}
+
+// ---------------------------------------------------------------- frame means of lerped-grid warps
+// acc[t, c] (+)= sum_n sample_n(lerp(base_n, target_n, alphas[t])) for a chunk of kMeanFrames frames per CTA, without writing
+// the (T, N, C, Ho, Wo) frames: a CTA owns a 32 x 8 output tile, stages base / target (tile + halo) of one sample at a time in
+// shared memory, and every thread keeps kMeanFrames x C sums in registers.  The samples are added in order, each value rounded
+// to the source dtype as the per-sample kernel stores it, so the sums equal a sequential fp32 sum of that kernel's frames.
+constexpr int kMeanFrames = 8;
+
+template <typename T, bool MIP, int C>
+__global__ void __launch_bounds__(kTileX * kTileY)
+warp_lerp_mean_kernel(float* __restrict__ acc, const T* __restrict__ src, const float* __restrict__ pyr,
+                      const ComposeParams cp, const __grid_constant__ WarpParams p, int frames, int tiles_x, int accumulate) {
+  __shared__ float2 sbase[kTileY + 2][kTileX + 2], starget[kTileY + 2][kTileX + 2];
+  const int tx = threadIdx.x % kTileX, ty = threadIdx.x / kTileX;
+  const int x0 = (blockIdx.x % tiles_x) * kTileX, y0 = (blockIdx.x / tiles_x) * kTileY;
+  const int ox = x0 + tx, oy = y0 + ty;
+  const bool live = ox < p.wo && oy < p.ho;
+  const int f0 = blockIdx.y * kMeanFrames;
+  const int nf = min(kMeanFrames, frames - f0);
+  float wt[kMeanFrames];
+  float s[kMeanFrames][C];
+#pragma unroll
+  for (int f = 0; f < kMeanFrames; ++f) {
+    wt[f] = (f < nf) ? __ldg(cp.alpha + f0 + f) : 0.f;
+#pragma unroll
+    for (int c = 0; c < C; ++c) s[f][c] = 0.f;
+  }
+  int hy = 0, hx = 0;
+  const bool halo = MIP && threadIdx.x < kRing;
+  if (halo) halo_slot(threadIdx.x, hy, hx);
+  const int64_t plane_px = p.ho * static_cast<int64_t>(p.wo) * 2;
+  const int64_t own = (static_cast<int64_t>(oy) * p.wo + ox) * 2;
+  const int64_t ring = (static_cast<int64_t>(min(max(y0 + hy, 0), p.ho - 1)) * p.wo + min(max(x0 + hx, 0), p.wo - 1)) * 2;
+  for (int64_t n = 0; n < p.n; ++n) {
+    const float* bn = cp.base + n * cp.base_stride;
+    const float* tg = cp.target + n * plane_px;
+    __syncthreads();   // the previous sample's tile has been read
+    if (live) {
+      sbase[ty + 1][tx + 1] = __ldg(reinterpret_cast<const float2*>(bn + own));
+      starget[ty + 1][tx + 1] = __ldg(reinterpret_cast<const float2*>(tg + own));
     }
-    out[(plane * p.ho + oy) * static_cast<int64_t>(p.wo) + ox] = Cvt<T>::from_f(o);
+    if (halo) {
+      sbase[hy + 1][hx + 1] = __ldg(reinterpret_cast<const float2*>(bn + ring));
+      starget[hy + 1][hx + 1] = __ldg(reinterpret_cast<const float2*>(tg + ring));
+    }
+    __syncthreads();
+    if (!live) continue;
+#pragma unroll
+    for (int f = 0; f < kMeanFrames; ++f) {
+      if (f >= nf) break;
+      auto grid_at = [&](int y, int x) {
+        return lerp_aten(sbase[y - y0 + 1][x - x0 + 1], starget[y - y0 + 1][x - x0 + 1], wt[f]);
+      };
+      const float2 g = grid_at(oy, ox);
+      const SampleGeom sg = sample_geom(g.x, g.y, p.hs, p.ws, p.pad_mode);
+      int l0 = 0, l1 = 0;
+      float w = 0.f;
+      if (MIP) {
+        const LevelInfo li = level_of_detail(grid_at, oy, ox, p.ho, p.wo, p.hs, p.ws, p.max_level, p.min_level);
+        l0 = li.l0; l1 = li.l1; w = li.w;
+      }
+#pragma unroll
+      for (int c = 0; c < C; ++c)
+        s[f][c] += Cvt<T>::to_f(Cvt<T>::from_f(sample_channel<T, MIP>(src, pyr, p, n * C + c, l0, l1, w, sg)));
+    }
+  }
+  if (!live) return;
+#pragma unroll
+  for (int f = 0; f < kMeanFrames; ++f) {
+    if (f >= nf) break;
+#pragma unroll
+    for (int c = 0; c < C; ++c) {
+      float* a = acc + ((static_cast<int64_t>(f0 + f) * C + c) * p.ho + oy) * static_cast<int64_t>(p.wo) + ox;
+      *a = accumulate ? *a + s[f][c] : s[f][c];
+    }
   }
 }
 
@@ -638,9 +751,11 @@ template <typename T>
 void sample_t(void* out, float* levels_out, const void* src, const float* pyramid, const ComposeParams& cp,
               const WarpParams& wp, int mode, unsigned ctas, int tiles_x, int tiles_y, cudaStream_t st) {
   using Kernel = void (*)(T*, float*, const T*, const float*, const ComposeParams, const WarpParams, int, int);
-  const Kernel kernels[2][3] = {
-      {warp_compose_fwd_kernel<T, false, 0>, warp_compose_fwd_kernel<T, false, 1>, warp_compose_fwd_kernel<T, false, 2>},
-      {warp_compose_fwd_kernel<T, true, 0>, warp_compose_fwd_kernel<T, true, 1>, warp_compose_fwd_kernel<T, true, 2>}};
+  const Kernel kernels[2][4] = {
+      {warp_compose_fwd_kernel<T, false, 0>, warp_compose_fwd_kernel<T, false, 1>, warp_compose_fwd_kernel<T, false, 2>,
+       warp_compose_fwd_kernel<T, false, 3>},
+      {warp_compose_fwd_kernel<T, true, 0>, warp_compose_fwd_kernel<T, true, 1>, warp_compose_fwd_kernel<T, true, 2>,
+       warp_compose_fwd_kernel<T, true, 3>}};
   kernels[wp.extra > 0][mode]<<<ctas, kTileX * kTileY, 0, st>>>(static_cast<T*>(out), levels_out,
                                                                static_cast<const T*>(src), pyramid, cp, wp, tiles_x, tiles_y);
 }
@@ -648,7 +763,7 @@ void sample_t(void* out, float* levels_out, const void* src, const float* pyrami
 int sample_forward(void* out, float* levels_out, const void* src, const float* pyramid, const ComposeParams& cp,
                    const WarpParams& wp, int mode, int dtype, const char* who, cudaStream_t st) {
   const int tiles_x = (wp.wo + kTileX - 1) / kTileX, tiles_y = (wp.ho + kTileY - 1) / kTileY;
-  const int64_t ctas = wp.n * tiles_x * static_cast<int64_t>(tiles_y);
+  const int64_t ctas = wp.n * tiles_x * static_cast<int64_t>(tiles_y) * (mode == 3 ? cp.frames : 1);
   if (ctas > 0x7fffffffLL) return fail(GG_ERR_BAD_ARG, "%s: too many tiles", who);
   switch (dtype) {
     case GG_F32: sample_t<float>(out, levels_out, src, pyramid, cp, wp, mode, ctas, tiles_x, tiles_y, st); break;
@@ -657,6 +772,26 @@ int sample_forward(void* out, float* levels_out, const void* src, const float* p
     default: return fail(GG_ERR_UNSUPPORTED, "%s: dtype %d not supported", who, dtype);
   }
   GG_CHECK_LAUNCH("warp_compose_fwd launch");
+  return GG_OK;
+}
+
+template <typename T, bool MIP>
+void lerp_mean_t(float* acc, const void* src, const float* pyramid, const ComposeParams& cp, const WarpParams& wp, dim3 grid,
+                 int tiles_x, int accumulate, cudaStream_t st) {
+  using Kernel = void (*)(float*, const T*, const float*, const ComposeParams, const WarpParams, int, int, int);
+  const Kernel kernels[4] = {warp_lerp_mean_kernel<T, MIP, 1>, warp_lerp_mean_kernel<T, MIP, 2>,
+                             warp_lerp_mean_kernel<T, MIP, 3>, warp_lerp_mean_kernel<T, MIP, 4>};
+  kernels[wp.c - 1]<<<grid, kTileX * kTileY, 0, st>>>(acc, static_cast<const T*>(src), pyramid, cp, wp, cp.frames, tiles_x,
+                                                      accumulate);
+}
+
+// shared argument checks of the two lerped-grid entry points
+int lerp_args(const char* who, const float* base, int64_t base_stride, const float* target, const float* alphas, int T,
+              int ho, int wo) {
+  if (T < 1) return fail(GG_ERR_BAD_ARG, "%s: T (the number of lerp weights) must be >= 1, got %d", who, T);
+  if (base_stride != 0 && base_stride != static_cast<int64_t>(ho) * wo * 2)
+    return fail(GG_ERR_BAD_ARG, "%s: base_stride must be 0 (one broadcast base grid) or ho*wo*2", who);
+  if (!base || !target || !alphas) return fail(GG_ERR_BAD_ARG, "%s: null grid or alphas", who);
   return GG_OK;
 }
 
@@ -799,6 +934,58 @@ int gg_stn_sample_forward(void* out, float* grid_out, float* delta_out, float* l
   cp.theta = theta; cp.low = low; cp.mask = mask; cp.identity = identity; cp.alpha = alpha;
   cp.lh = lh; cp.lw = lw; cp.s = s; cp.grid_out = grid_out; cp.delta_out = delta_out;
   return sample_forward(out, levels_out, src, pyramid, cp, wp, mode, dtype, "stn_sample", static_cast<cudaStream_t>(stream));
+}
+
+int gg_mipmap_warp_lerp_forward(void* out, float* grid_out, const void* src, const float* pyramid, const float* base,
+                                int64_t base_stride, const float* target, const float* alphas, int T, int dtype, int64_t N,
+                                int C, int hs, int ws, int ho, int wo, int extra_levels, float max_level, float min_level,
+                                int padding_mode, void* stream) {
+  WarpParams wp;
+  int rc = fill_params(&wp, N, C, hs, ws, ho, wo, padding_mode, extra_levels, max_level, min_level);
+  if (rc != GG_OK) return rc;
+  rc = lerp_args("mipmap_warp_lerp_forward", base, base_stride, target, alphas, T, ho, wo);
+  if (rc != GG_OK) return rc;
+  const int64_t total = N * ho * static_cast<int64_t>(wo);
+  if (total == 0 || C == 0) return GG_OK;
+  if (!out || !src || (extra_levels > 0 && !pyramid)) return fail(GG_ERR_BAD_ARG, "mipmap_warp_lerp_forward: null tensor");
+  ComposeParams cp{};
+  cp.base = base; cp.base_stride = base_stride; cp.target = target; cp.alpha = alphas; cp.frames = T; cp.grid_out = grid_out;
+  return sample_forward(out, nullptr, src, pyramid, cp, wp, 3, dtype, "mipmap_warp_lerp_forward",
+                        static_cast<cudaStream_t>(stream));
+}
+
+int gg_mipmap_warp_lerp_mean(float* acc, const void* src, const float* pyramid, const float* base, int64_t base_stride,
+                             const float* target, const float* alphas, int T, int dtype, int64_t N, int C, int hs, int ws,
+                             int ho, int wo, int extra_levels, float max_level, float min_level, int padding_mode,
+                             int accumulate, void* stream) {
+  WarpParams wp;
+  int rc = fill_params(&wp, N, C, hs, ws, ho, wo, padding_mode, extra_levels, max_level, min_level);
+  if (rc != GG_OK) return rc;
+  rc = lerp_args("mipmap_warp_lerp_mean", base, base_stride, target, alphas, T, ho, wo);
+  if (rc != GG_OK) return rc;
+  if (C < 1 || C > 4) return fail(GG_ERR_UNSUPPORTED, "mipmap_warp_lerp_mean: 1 <= C <= 4 channels, got %d", C);
+  if (!acc || (N > 0 && !src) || (N > 0 && extra_levels > 0 && !pyramid))
+    return fail(GG_ERR_BAD_ARG, "mipmap_warp_lerp_mean: null tensor");
+  if (static_cast<int64_t>(ho) * wo == 0) return GG_OK;
+  const int tiles_x = (wo + kTileX - 1) / kTileX, tiles_y = (ho + kTileY - 1) / kTileY;
+  const int64_t chunks = (T + kMeanFrames - 1) / kMeanFrames;
+  if (static_cast<int64_t>(tiles_x) * tiles_y > 0x7fffffffLL || chunks > 65535)
+    return fail(GG_ERR_BAD_ARG, "mipmap_warp_lerp_mean: too many tiles or frames");
+  ComposeParams cp{};
+  cp.base = base; cp.base_stride = base_stride; cp.target = target; cp.alpha = alphas; cp.frames = T;
+  const dim3 grid(static_cast<unsigned>(tiles_x * tiles_y), static_cast<unsigned>(chunks));
+  auto st = static_cast<cudaStream_t>(stream);
+  const bool mip = extra_levels > 0;
+  switch (dtype) {
+    case GG_F32: (mip ? lerp_mean_t<float, true> : lerp_mean_t<float, false>)(acc, src, pyramid, cp, wp, grid, tiles_x, accumulate, st); break;
+    case GG_F16: (mip ? lerp_mean_t<__half, true> : lerp_mean_t<__half, false>)(acc, src, pyramid, cp, wp, grid, tiles_x, accumulate, st); break;
+    case GG_BF16:
+      (mip ? lerp_mean_t<__nv_bfloat16, true> : lerp_mean_t<__nv_bfloat16, false>)(acc, src, pyramid, cp, wp, grid, tiles_x, accumulate, st);
+      break;
+    default: return fail(GG_ERR_UNSUPPORTED, "mipmap_warp_lerp_mean: dtype %d not supported", dtype);
+  }
+  GG_CHECK_LAUNCH("warp_lerp_mean launch");
+  return GG_OK;
 }
 
 int gg_mipmap_warp_backward(float* grad_src, float* grad_pyramid, float* grad_grid, const void* grad_out,

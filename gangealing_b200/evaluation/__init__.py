@@ -1,8 +1,10 @@
 """Evaluation of a trained STN: PCK-Transfer (reference applications/pck.py), the test-time flip decision
-(applications/__init__.py) and flow-smoothness scores (applications/flow_scores.py)."""
+(applications/__init__.py), flow-smoothness scores (applications/flow_scores.py) and the congealing visualisations
+(applications/vis_correspondence.py, propagate_to_images.py)."""
 from .flips import determine_flips
 from .flow_scores import filter_dataset, flow_scores, get_high_score_indices
 from .pck import pck_transfer, pck_transfer_batch
+from .visuals import average_congealed_image, congealing_average_frames, smooth_congealing
 
-__all__ = ["determine_flips", "filter_dataset", "flow_scores", "get_high_score_indices", "pck_transfer",
-           "pck_transfer_batch"]
+__all__ = ["average_congealed_image", "congealing_average_frames", "determine_flips", "filter_dataset", "flow_scores",
+           "get_high_score_indices", "pck_transfer", "pck_transfer_batch", "smooth_congealing"]

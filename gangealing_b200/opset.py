@@ -20,6 +20,7 @@ def cuda_ops():
         from .splat2d import nn_argmin as _nn_argmin
         from .splat2d import splat2d as _splat2d
         from .splat2d import splat2d_lookup as _splat2d_lookup
+        from .splat2d import track_points_lerp as _track_points_lerp
         from .splat2d import laplacian_blend as _laplacian_blend
         from .op import feature_distance as _fd
         from .op import vgg_pool as _vp
@@ -53,5 +54,8 @@ def cuda_ops():
             tv_per_sample=_ev.tv_per_sample,              # match_flows / flow_scores: per-sample smoothness, one launch
             pck_transfer_points=_ev.pck_transfer_points,  # PCK-Transfer: congeal + search + lookup + score, one call
             batch_gram=_pca.batch_gram,                   # IncrementalPCA's per-batch means + centred Grams, fp64 DMMA
+            mipmap_warp_lerp=_smp.mipmap_warp_lerp,       # congealing animation: T lerped-grid warps from one pyramid
+            mipmap_warp_lerp_mean=_smp.mipmap_warp_lerp_mean,   # ... and their per-frame batch sums, frames never written
+            track_points_lerp=_track_points_lerp,         # dense point tracking over a stage's frames, one launch
         )
     return _cached

@@ -2,9 +2,10 @@
 import torch.nn as nn
 
 from .blend import LaplacianBlender, laplacian_blend, splat_points
-from .functional import nn_argmin, splat2d, splat2d_lookup
+from .functional import nn_argmin, splat2d, splat2d_lookup, track_points_lerp
 
-__all__ = ["Splat2D", "splat2d", "splat2d_lookup", "nn_argmin", "laplacian_blend", "LaplacianBlender", "splat_points"]
+__all__ = ["Splat2D", "splat2d", "splat2d_lookup", "nn_argmin", "track_points_lerp", "laplacian_blend", "LaplacianBlender",
+           "splat_points"]
 
 
 class Splat2D(nn.Module):

@@ -8,7 +8,7 @@ import torch.autograd as ag
 
 from .. import _lib
 
-__all__ = ["splat2d", "splat2d_lookup", "nn_argmin"]
+__all__ = ["splat2d", "splat2d_lookup", "nn_argmin", "track_points_lerp"]
 
 
 class Splat2DFunction(ag.Function):
@@ -92,3 +92,34 @@ def nn_argmin(grid, points):
     _lib.check(lib.gg_nn_argmin(index.data_ptr(), ws.data_ptr(), g.data_ptr(), pts.data_ptr(), n, p, g.size(1), _lib.stream()),
                "gg_nn_argmin")
     return index
+
+
+@torch.no_grad()
+def track_points_lerp(base, target, alphas, points, centers, patch_size):
+    """Dense point tracking of the congealing animation (reference vis_correspondence.py:59-114, looped over the frames of
+    smoothly_sample_image :183-205) in one launch: frame t searches the patch_size^2 window around each point's centre of
+    pad_grid(base.lerp(target, alphas[t])) for the entry nearest to the point and carries it to frame t + 1.
+    base / target (N, H, H, 2); alphas (T,); points (N, P, 2) normalised; centers (N, P, 2) integer pixel centres before
+    frame 0, each in [-1, H] (checked here with one host sync).  Inference only.
+    -> (track (T, N, P, 2) int64, the last frame's centres (N, P, 2) int64)."""
+    _lib.require_cuda(base, target, alphas, points, centers)
+    if target.dim() != 4 or target.size(-1) != 2 or base.shape != target.shape:
+        raise RuntimeError("track_points_lerp: base and target must both be (N, H, W, 2)")
+    n, h, w = target.shape[:3]
+    if points.dim() != 3 or points.size(0) != n or points.size(2) != 2 or centers.shape != points.shape:
+        raise RuntimeError("track_points_lerp: points and centers must be (N, P, 2) with N = %d" % n)
+    if alphas.dim() != 1:
+        raise RuntimeError("track_points_lerp: alphas must be (T,)")
+    if centers.is_floating_point():
+        raise RuntimeError("track_points_lerp: centers must be integer pixel coordinates")
+    c = centers.to(torch.int64).clone(memory_format=torch.contiguous_format)
+    if c.numel() and bool(((c < -1) | (c[..., 0:1] > w) | (c[..., 1:2] > h)).any()):
+        raise RuntimeError("track_points_lerp: patch centres must lie in [-1, W] x [-1, H] (the padded grid)")
+    b, tg = base.float().contiguous(), target.float().contiguous()
+    al, pts = alphas.float().contiguous(), points.float().contiguous()
+    t = al.numel()
+    track = torch.empty((t, n, points.size(1), 2), dtype=torch.int64, device=base.device)
+    _lib.check(_lib.load().gg_track_points_lerp(track.data_ptr(), c.data_ptr(), b.data_ptr(), tg.data_ptr(), al.data_ptr(),
+                                                pts.data_ptr(), t, n, points.size(1), h, w, int(patch_size), _lib.stream()),
+               "gg_track_points_lerp")
+    return track, c

@@ -206,6 +206,80 @@ def mipmap_warp(inputs, grid, max_num_levels=8, min_level=0.0, padding_mode="bor
     return out, levels
 
 
+def _lerp_operands(who, inputs, base, target, alphas):
+    """Checked, dense fp32 operands of the lerped-grid sampler: -> (x, base, base_stride, target, alphas, ho, wo)."""
+    _lib.require_cuda(inputs, base, target, alphas)
+    if inputs.dim() != 4:
+        raise RuntimeError("%s: expected inputs (N, C, H, W), got %s" % (who, tuple(inputs.shape)))
+    n = inputs.shape[0]
+    if target.dim() != 4 or target.shape[0] != n or target.shape[-1] != 2:
+        raise RuntimeError("%s: target must be (N, Ho, Wo, 2) with N = %d, got %s" % (who, n, tuple(target.shape)))
+    ho, wo = target.shape[1], target.shape[2]
+    if base.dim() != 4 or base.shape[1:] != target.shape[1:] or base.shape[0] not in (1, n):
+        raise RuntimeError("%s: base must be (N or 1, %d, %d, 2), got %s" % (who, ho, wo, tuple(base.shape)))
+    if alphas.dim() != 1 or alphas.numel() < 1:
+        raise RuntimeError("%s: alphas must be a non-empty (T,) tensor" % who)
+    b = base.float().contiguous()
+    stride = 0 if (b.shape[0] == 1 and n != 1) else ho * wo * 2
+    return (inputs.contiguous(), b, stride, target.float().contiguous(), alphas.float().contiguous(), ho, wo)
+
+
+def _pyramid(x, extra):
+    lib = _lib.load()
+    n, c, hs, ws = x.shape
+    if extra == 0:
+        return None
+    elems = lib.gg_mipmap_pyramid_elems(n * c, hs, ws, extra)
+    if elems < 0:
+        raise RuntimeError("MipmapWarp: a %dx%d source cannot host %d mip levels" % (hs, ws, extra))
+    pyr = torch.empty(max(int(elems), 1), dtype=torch.float32, device=x.device)
+    _lib.check(lib.gg_mipmap_build(pyr.data_ptr(), x.data_ptr(), _lib.dtype_code(x), n * c, hs, ws, extra, _lib.stream()),
+               "gg_mipmap_build")
+    return pyr
+
+
+@torch.no_grad()
+def mipmap_warp_lerp(inputs, base, target, alphas, max_num_levels=8, min_level=0.0, padding_mode="border"):
+    """`MipmapWarp(max_num_levels)(inputs, base.lerp(target, alphas[t]))` for every lerp weight at once (reference
+    vis_correspondence.py:183-205, :335-380), from one pyramid: base (N or 1, Ho, Wo, 2), target (N, Ho, Wo, 2), alphas
+    (T,).  Inference only.  -> (out (T, N, C, Ho, Wo) in inputs' dtype, grids (T, N, Ho, Wo, 2) fp32)."""
+    x, b, stride, tg, al, ho, wo = _lerp_operands("mipmap_warp_lerp", inputs, base, target, alphas)
+    n, c, hs, ws = x.shape
+    max_level, min_level, extra = clamp_levels(hs, ws, max_num_levels, min_level)
+    t = al.numel()
+    out = torch.empty((t, n, c, ho, wo), dtype=x.dtype, device=x.device)
+    grids = torch.empty((t, n, ho, wo, 2), dtype=torch.float32, device=x.device)
+    pyr = _pyramid(x, extra)
+    rc = _lib.load().gg_mipmap_warp_lerp_forward(out.data_ptr(), grids.data_ptr(), x.data_ptr(), _lib.ptr(pyr), b.data_ptr(),
+                                                 stride, tg.data_ptr(), al.data_ptr(), t, _lib.dtype_code(x), n, c, hs, ws, ho,
+                                                 wo, extra, max_level, min_level, _pad_code(padding_mode), _lib.stream())
+    _lib.check(rc, "gg_mipmap_warp_lerp_forward")
+    return out, grids
+
+
+@torch.no_grad()
+def mipmap_warp_lerp_mean(inputs, base, target, alphas, acc=None, max_num_levels=8, min_level=0.0, padding_mode="border"):
+    """Per-frame sums over the batch of `mipmap_warp_lerp`'s frames without materialising them: acc (T, C, Ho, Wo) fp32
+    += sum_n out[t, n] (the samples added in order; acc None: a new tensor holding the sums).  C <= 4.  Inference only.
+    -> acc."""
+    x, b, stride, tg, al, ho, wo = _lerp_operands("mipmap_warp_lerp_mean", inputs, base, target, alphas)
+    n, c, hs, ws = x.shape
+    t = al.numel()
+    accumulate = acc is not None
+    if acc is None:
+        acc = torch.empty((t, c, ho, wo), dtype=torch.float32, device=x.device)
+    elif acc.shape != (t, c, ho, wo) or acc.dtype != torch.float32 or not acc.is_contiguous():
+        raise RuntimeError("mipmap_warp_lerp_mean: acc must be a contiguous fp32 (%d, %d, %d, %d) tensor" % (t, c, ho, wo))
+    _lib.require_cuda(acc)
+    max_level, min_level, extra = clamp_levels(hs, ws, max_num_levels, min_level)
+    pyr = _pyramid(x, extra)
+    rc = _lib.load().gg_mipmap_warp_lerp_mean(acc.data_ptr(), x.data_ptr(), _lib.ptr(pyr), b.data_ptr(), stride, tg.data_ptr(),
+                                              al.data_ptr(), t, _lib.dtype_code(x), n, c, hs, ws, ho, wo, extra, max_level,
+                                              min_level, _pad_code(padding_mode), int(accumulate), _lib.stream())
+    _lib.check(rc, "gg_mipmap_warp_lerp_mean")
+    return acc
+
+
 class _TentDownsample(Function):
     """BilinearDownsample as one gather kernel (csrc/resample.cu); backward = its exact adjoint."""
 

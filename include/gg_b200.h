@@ -177,6 +177,24 @@ GG_API int gg_mipmap_warp_backward(float* grad_src, float* grad_pyramid, float* 
  * evaluated by the same device functions as the forward sampler of gg_mipmap_warp_forward / gg_stn_sample_forward. */
 GG_API int gg_warp_sample_indices(int32_t* indices, const float* grid, int64_t N, int hs, int ws, int ho, int wo,
                                   float max_level, float min_level, int padding_mode, void* stream);
+/* Congealing animations: vis_correspondence.py:183-205 (smoothly_sample_image) and :335-380 (create_average_image), i.e.
+ * warper(data, base.lerp(target, alpha_t)) for T lerp weights at once.  The grid of frame t, sample n is
+ * lerp(base[n], target[n], alphas[t]) with torch.lerp's formula (bitwise torch.lerp on the device); the level of detail and
+ * the trilinear sample are gg_mipmap_warp_forward's.  One pyramid (gg_mipmap_build of src) serves all T frames.
+ *   base (N or 1, ho, wo, 2) fp32: base_stride = ho*wo*2, or 0 for one broadcast grid; target (N, ho, wo, 2) fp32;
+ *   alphas (T,) fp32 on the device; T >= 1.
+ *   gg_mipmap_warp_lerp_forward: out (T, N, C, ho, wo) `dtype`; grid_out (T, N, ho, wo, 2) fp32 or NULL.
+ *   gg_mipmap_warp_lerp_mean: acc (T, C, ho, wo) fp32, s = 0; for n = 0..N-1 in order: s += sample_n(frame t) (each value
+ *     rounded to `dtype` as gg_mipmap_warp_lerp_forward stores it); acc = accumulate ? acc + s : s.  No atomics: bitwise
+ *     reproducible, and bitwise a sequential fp32 sum of gg_mipmap_warp_lerp_forward's frames.  1 <= C <= 4. */
+GG_API int gg_mipmap_warp_lerp_forward(void* out, float* grid_out, const void* src, const float* pyramid, const float* base,
+                                       int64_t base_stride, const float* target, const float* alphas, int T, int dtype,
+                                       int64_t N, int C, int hs, int ws, int ho, int wo, int extra_levels, float max_level,
+                                       float min_level, int padding_mode, void* stream);
+GG_API int gg_mipmap_warp_lerp_mean(float* acc, const void* src, const float* pyramid, const float* base, int64_t base_stride,
+                                    const float* target, const float* alphas, int T, int dtype, int64_t N, int C, int hs,
+                                    int ws, int ho, int wo, int extra_levels, float max_level, float min_level,
+                                    int padding_mode, int accumulate, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Flow composition of the flow STN head -- replaces upsample_flow + identity add + apply_affine + alpha lerp
@@ -390,6 +408,18 @@ GG_API int gg_tent_downsample_backward(float* grad_in, const float* grad_out, co
 GG_API int64_t gg_nn_argmin_workspace(int64_t N, int64_t P);
 GG_API int gg_nn_argmin(int64_t* index, void* workspace, const float* grid, const float* points, int64_t N, int64_t P, int HW,
                         void* stream);
+/* Dense point tracking of the congealing animation: vis_correspondence.py:59-114 (pad_grid + nearest_neighbor_within_patch)
+ * looped over frames as smoothly_sample_image (:183-205) does, one launch for all T frames (no Unfold tensor).
+ * Frame t searches the patch x patch window around each point's centre of pad_grid(lerp(base, target, alphas[t])) -- the
+ * (H+2) x (W+2) grid with the linear-extrapolation ring; window positions beyond it are Unfold's (0, 0) zero padding and
+ * stay candidates -- with the expanded distance |p|^2 + |g|^2 - 2 g.p (separately rounded; first minimum in row-major
+ * window order wins) and carries the result as the next frame's centre.  The result index is flat_centre + dx + (H+2) dy,
+ * unravelled over (H+2, W+2) with floor division (a window leaving the padded grid wraps around) and minus 1.
+ *   track (T, N, P, 2) int64 (x, y) per frame; centers (N, P, 2) int64 IN: centres before frame 0 (each in [-1, H]; the
+ *   caller validates), OUT: the last frame's result; points (N, P, 2) fp32 normalised; base / target (N, H, W, 2) fp32
+ *   with H == W >= 2 (the reference indexes with grid.size(1) as the row stride); patch odd >= 1; alphas (T,) device. */
+GG_API int gg_track_points_lerp(int64_t* track, int64_t* centers, const float* base, const float* target, const float* alphas,
+                                const float* points, int T, int64_t N, int64_t P, int H, int W, int patch, void* stream);
 GG_API int gg_splat2d_lookup_forward(float* out, float* points_out, void* workspace, const float* input, const float* grid,
                                      const float* query, const float* values, const float* sigma, int64_t N, int64_t P,
                                      int C, int H, int W, int grid_h, int grid_w, float unnorm_k, float unnorm_m,

@@ -1,0 +1,137 @@
+"""Time the congealing visualisations on the GPU against the reference's per-frame formulation on this repository's
+cuda_ops() mirror.  Seeded weights (flow 128, channel multiplier 0.5) and images.
+
+    python tools/visbench.py [--frames-window 4] [--n-mean 1000]
+
+Average-image animation, 512^2 source and output, two STN stages x 240 frames, batches of 50:
+  * the reference formulation (create_average_image: flip inference + STN + lerp + warp + sum, again for every frame), per
+    frame and per batch of 50, timed over a window of frames (a per-frame figure, not a total);
+  * congealing_average_frames end to end at n_mean images;
+  * the mean kernel (gg_mipmap_warp_lerp_mean) per (sample, frame), with its DRAM bytes.
+Point tracking, N = 4, P = 40000, patch 9, 512^2 grids, 240 frames: track_points_lerp against the per-frame Unfold
+composition (oracle.vis.nearest_neighbor_within_patch on the device).  Needs a CUDA device.
+"""
+import argparse
+import os
+import subprocess
+import sys
+import time
+
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+from gangealing_b200.evaluation import congealing_average_frames  # noqa: E402
+from gangealing_b200.evaluation import visuals as V  # noqa: E402
+from gangealing_b200.stn import get_stn  # noqa: E402
+from gangealing_b200.stn.sampling import MipmapWarp, mipmap_warp_lerp_mean  # noqa: E402
+from gangealing_b200.splat2d import track_points_lerp  # noqa: E402
+from oracle import opset  # noqa: E402
+from oracle import vis as OV  # noqa: E402
+
+
+def _card():
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=30).stdout.strip()
+    except Exception as exc:  # the timing does not depend on it
+        q = "nvidia-smi unavailable (%s)" % exc
+    return q or torch.cuda.get_device_name()
+
+
+def _events(fn, reps=1):
+    torch.cuda.synchronize()
+    start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    start.record()
+    for _ in range(reps):
+        fn()
+    end.record()
+    end.synchronize()
+    return start.elapsed_time(end) / reps
+
+
+@torch.no_grad()
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--frames-window", type=int, default=4)
+    ap.add_argument("--n-mean", type=int, default=1000)
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("visbench: needs a CUDA device")
+    dev = "cuda"
+    print("card: %s" % _card())
+    res, batch, length = 512, 50, 240
+    t = opset.fill_parameters(get_stn(["similarity", "flow"], flow_size=128, supersize=res, channel_multiplier=0.5).eval(),
+                              51, gain=0.6).to(dev)
+    g = torch.Generator().manual_seed(0)
+    data = torch.randn(batch, 3, res, res, generator=g).to(dev)
+
+    # the reference formulation: every frame re-runs the flips and the STN over the batch, then lerps, warps and sums
+    identity = V._identity(1, res, data)
+    warper = MipmapWarp(3.5)
+    alphas = V.cosine_alphas(length, dev)
+
+    def ref_frame(i):
+        flipped, flips, policy = V.determine_flips(t, None, data)
+        _, grids = t(flipped, warp_policy=policy, return_intermediates=True)
+        grid = V._resize(V.flip_grid(grids[1], flips), res)
+        base = V._resize(V.flip_grid(grids[0], flips), res)
+        return warper(data, base.lerp(grid, alphas[i])).sum(dim=0, keepdim=True)
+
+    ref_frame(0)
+    w = args.frames_window
+    ms = _events(lambda: [ref_frame(i) for i in range(w)]) / w
+    print("reference formulation (per-frame flips + STN + warp + sum), batch %d at %d^2: %.1f ms per frame per batch "
+          "(window of %d frames)" % (batch, res, ms, w))
+
+    # end to end
+    n_batches = args.n_mean // batch
+    batches = [torch.randn(batch, 3, res, res, generator=g).to(dev) for _ in range(min(n_batches, 4))]
+    loader = [batches[i % len(batches)] for i in range(n_batches)]
+    congealing_average_frames(t, loader[:1], batch, length=4, vis_in_stages=True, output_resolution=res)   # warm-up
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    frames = congealing_average_frames(t, loader, args.n_mean, length=length, vis_in_stages=True, output_resolution=res)
+    torch.cuda.synchronize()
+    e2e = time.perf_counter() - t0
+    print("congealing_average_frames: n_mean %d, 2 stages x %d frames at %d^2: %.2f s end to end (%s)" %
+          (args.n_mean, length, res, e2e, tuple(frames.shape)))
+    del frames
+
+    # the mean kernel alone: one stage of one batch
+    flipped, flips, policy = V.determine_flips(t, None, data)
+    _, grids = t(flipped, warp_policy=policy, return_intermediates=True)
+    target = V._resize(V.flip_grid(grids[1], flips), res)
+    base = V._resize(V.flip_grid(grids[0], flips), res)
+    acc = torch.zeros(length, 3, res, res, device=dev)
+    mipmap_warp_lerp_mean(data, base, target, alphas, acc, 3.5)
+    kms = _events(lambda: mipmap_warp_lerp_mean(data, base, target, alphas, acc, 3.5), 3)
+    per = kms * 1e3 / (batch * length)
+    dram = 4 * (batch * 3 * res * res * 4 / 3 + 2 * batch * res * res * 2 + 2 * length * 3 * res * res)   # src + pyramid, grids, acc
+    print("mean kernel: %.2f ms per call (%d samples x %d frames) = %.2f us per (sample, frame); DRAM bytes %.2f GB -> "
+          "%.0f GB/s (%.1f%% of 3.35 TB/s): bound by the per-pixel gathers (L1/L2), not DRAM" %
+          (kms, batch, length, per, dram / 1e9, dram / kms / 1e6, 100 * dram / kms / 1e6 / 3350))
+
+    # point tracking
+    n, p, ps = 4, 40000, 9
+    tb, tt = base[:n].contiguous(), target[:n].contiguous()
+    pts = torch.rand(n, p, 2, generator=g).to(dev) * 1.6 - 0.8
+    centers = torch.randint(0, res, (n, p, 2), generator=g).to(dev)
+    track_points_lerp(tb, tt, alphas, pts, centers, ps)
+    kt = _events(lambda: track_points_lerp(tb, tt, alphas, pts, centers, ps), 3)
+    c = centers
+
+    def unfold_frames():
+        nonlocal c
+        for i in range(w):
+            c = OV.nearest_neighbor_within_patch(tb.lerp(tt, alphas[i]), pts, c, ps)
+
+    unfold_frames()
+    uf = _events(unfold_frames) / w
+    print("tracker: N %d, P %d, patch %d, %d^2, %d frames: %.2f ms per launch (%.3f ms per frame); per-frame Unfold "
+          "composition %.2f ms per frame (window of %d frames)" % (n, p, ps, res, length, kt, kt / length, uf, w))
+
+
+if __name__ == "__main__":
+    main()

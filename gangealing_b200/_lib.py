@@ -51,7 +51,10 @@ SIGNATURES = {
     "gg_bias_act_backward_nhwc": (_I, [_P] * 5 + [_I, _F, _F, _L, _I, _L, _P]),
     "gg_blur_nhwc_workspace": (_L, [_I, _L] + [_I] * 9),
     "gg_blur_nhwc": (_I, [_P] * 12 + [_I, _L] + [_I] * 12 + [_F, _F, _P]),
+    "gg_blur_nhwc_mask": (_I, [_P] * 9 + [_I, _L] + [_I] * 11 + [_F, _F, _P]),
     "gg_styled_tail_nhwc": (_I, [_P] * 12 + [_I, _I, _F, _F, _L, _I, _L, _P]),
+    "gg_styled_tail_mask_nhwc": (_I, [_P] * 12 + [_I, _I, _F, _F, _L, _I, _L, _P]),
+    "gg_styled_tail_backward_mask_nhwc": (_I, [_P] * 7 + [_I, _F, _F, _L, _I, _L, _P]),
     "gg_styled_tail_backward_workspace": (_L, [_I, _L, _I, _L]),
     "gg_styled_tail_backward_nhwc": (_I, [_P] * 12 + [_I, _F, _F, _L, _I, _L, _L, _P]),
     "gg_tent_downsample_forward": (_I, [_P] * 4 + [_L, _I, _I, _I, _I, _P]),

@@ -153,6 +153,37 @@ __device__ __forceinline__ void stg_stream16(void* p, const uint4& u) {
   asm volatile("st.global.L1::no_allocate.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(u.x), "r"(u.y), "r"(u.z), "r"(u.w) : "memory");
 }
 
+// ---------------------------------------------------------------- sign mask of a channels-last activation
+// One bit per element, `stored value > 0` (what lrelu' tests in the backward kernels), packed along the channels: word w of
+// a pixel holds channels 32w .. 32w+31, bit = channel & 31; the tensor is (N, H, W, C/32) uint32.  A backward pass that
+// needs no reduction over the activation reads the mask (1/32 or 1/16 of the bytes) instead of the activation.
+// SignFloor<T>::v: the largest fp32 value whose STORED form is not positive.  bf16 rounds (0, 2^-134] to zero.
+template <typename T> struct SignFloor { static constexpr float v = 0.f; };
+template <> struct SignFloor<__nv_bfloat16> { static constexpr float v = 0x1p-134f; };
+
+template <typename T, int V>
+__device__ __forceinline__ uint32_t sign_bits(const float (&o)[V]) {
+  uint32_t m = 0u;
+#pragma unroll
+  for (int k = 0; k < V; ++k) m |= (o[k] > SignFloor<T>::v ? 1u : 0u) << k;
+  return m;
+}
+// The 32 / V adjacent lanes that own one word's channels (lane `cq` owns channels cq*V ..) combine their bits; every lane of
+// `lanes` must call.  The word is complete in all of them; the lane with (cq*V) % 32 == 0 stores it.
+template <int V>
+__device__ __forceinline__ uint32_t sign_word(uint32_t bits, int cq, unsigned lanes) {
+  constexpr int L = 32 / V;
+  uint32_t w = bits << (V * (cq & (L - 1)));
+#pragma unroll
+  for (int m = L / 2; m >= 1; m >>= 1) w |= __shfl_xor_sync(lanes, w, m);
+  return w;
+}
+// the V bits of channel vector `cq` (channels cq*V ..) of a pixel whose mask words start at `px`
+template <int V>
+__device__ __forceinline__ uint32_t sign_load(const uint32_t* px, int cq) {
+  return __ldg(px + (cq * V >> 5)) >> (cq * V & 31);
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -336,6 +336,8 @@ __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* t
 //   FAST    (MODE 1) the gain-folded epilogue `max(T, T*slope)` is valid for the launch (gain > 0, 0 <= slope <= 1 or linear):
 //           a compile-time variant -- as a run-time flag the compiler predicated BOTH epilogues into the row loop (FSETP /
 //           FSEL / FMUL of the general path: 16 % of the issue slots of the bf16 kernel, which is issue-bound)
+//   MODE 3  MODE 1 whose `out` receives the sign mask of o (common.cuh), (N, H, W, C/32) uint32, instead of o: all that a
+//           backward pass without reductions over o needs of it
 template <typename T, int MODE, bool SEP, bool FAST = false>
 __global__ void __launch_bounds__(kT, 2)
 blur_nhwc_kernel(T* __restrict__ out, T* __restrict__ out2, const __grid_constant__ CUtensorMap tmap,
@@ -345,7 +347,8 @@ blur_nhwc_kernel(T* __restrict__ out, T* __restrict__ out2, const __grid_constan
                  float* __restrict__ partial, BlurNhwcParams p) {
   using G = BlurGeom<T>;
   constexpr int V = G::V, CB = G::CB, COLS = G::COLS, BX = G::BX, TW = G::TW;
-  constexpr bool FUSED = MODE == 1;
+  constexpr bool FUSED = MODE == 1 || MODE == 3;
+  constexpr bool MASK = MODE == 3;
   extern __shared__ __align__(128) unsigned char tiles_raw[];
   T* tiles = reinterpret_cast<T*>(tiles_raw);
   __shared__ uint64_t full_bar[kNS];
@@ -602,8 +605,14 @@ blur_nhwc_kernel(T* __restrict__ out, T* __restrict__ out2, const __grid_constan
               a4[k] = t;
               o2[k] = __fmul_rn(t, sq[k]);
             }
+            uint32_t word = 0u;
+            if (MASK) word = sign_word<V>(sign_bits<T>(a4), cq, 0xffffffffu);   // `ro` is uniform: every lane is here
             if (okc[j]) {
-              if (out) *reinterpret_cast<uint4*>(out + ooff) = ChanVec<T>::pack(a4);
+              if (MASK) {
+                if ((cq * V & 31) == 0) reinterpret_cast<uint32_t*>(out)[ooff >> 5] = word;
+              } else if (out) {
+                *reinterpret_cast<uint4*>(out + ooff) = ChanVec<T>::pack(a4);
+              }
               if (out2) *reinterpret_cast<uint4*>(out2 + ooff) = ChanVec<T>::pack(o2);
             }
           } else if (MODE == 2) {
@@ -882,7 +891,7 @@ static int launch_blur(void* out, void* out2, const void* in, const float* kerne
                        const float* noise_weight, const float* bias, const float* row_scale, const float* scale2,
                        const void* mul, float* row_dot, void* workspace, int64_t N, int C, int in_h, int in_w, int kernel_h,
                        int kernel_w, int separable, int pad_x0, int pad_x1, int pad_y0, int pad_y1, int mode, int act,
-                       float alpha, float scale, void* stream, int dtype) {
+                       float alpha, float scale, void* stream, int dtype, bool out_is_mask) {
   using G = BlurGeom<T>;
   BlurPlan pl;
   int rc = blur_plan(&pl, dtype, N, C, in_h, in_w, kernel_h, kernel_w, pad_x0, pad_x1, pad_y0, pad_y1);
@@ -928,15 +937,19 @@ static int launch_blur(void* out, void* out2, const void* in, const float* kerne
   static DeviceOnce configured;
   if (configured.needed()) {
     cudaError_t e = cudaSuccess;
-    const void* kernels[8] = {reinterpret_cast<const void*>(blur_nhwc_kernel<T, 0, true>),
+    const void* kernels[12] = {reinterpret_cast<const void*>(blur_nhwc_kernel<T, 0, true>),
                               reinterpret_cast<const void*>(blur_nhwc_kernel<T, 0, false>),
                               reinterpret_cast<const void*>(blur_nhwc_kernel<T, 1, true, false>),
                               reinterpret_cast<const void*>(blur_nhwc_kernel<T, 1, false, false>),
                               reinterpret_cast<const void*>(blur_nhwc_kernel<T, 1, true, true>),
                               reinterpret_cast<const void*>(blur_nhwc_kernel<T, 1, false, true>),
+                              reinterpret_cast<const void*>(blur_nhwc_kernel<T, 3, true, false>),
+                              reinterpret_cast<const void*>(blur_nhwc_kernel<T, 3, false, false>),
+                              reinterpret_cast<const void*>(blur_nhwc_kernel<T, 3, true, true>),
+                              reinterpret_cast<const void*>(blur_nhwc_kernel<T, 3, false, true>),
                               reinterpret_cast<const void*>(blur_nhwc_kernel<T, 2, true>),
                               reinterpret_cast<const void*>(blur_nhwc_kernel<T, 2, false>)};
-    for (int i = 0; i < 8 && e == cudaSuccess; ++i)
+    for (int i = 0; i < 12 && e == cudaSuccess; ++i)
       e = cudaFuncSetAttribute(kernels[i], cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
     if (e != cudaSuccess) return cuda_fail(e, "blur_nhwc smem opt-in");
     configured.done();
@@ -948,7 +961,11 @@ static int launch_blur(void* out, void* out2, const void* in, const float* kerne
   blur_nhwc_kernel<T, M_, S_, F_><<<grid, kT, smem, st>>>(static_cast<T*>(out), static_cast<T*>(out2), tmap, kernel, kernel_h, \
                                                          kernel_w, noise, noise_weight, bias, row_scale, scale2,     \
                                                          static_cast<const T*>(mul), partial, p)
-  if (mode == 1) {
+  if (mode == 1 && out_is_mask) {
+    if (fast) { if (separable) GG_BLUR(3, true, true); else GG_BLUR(3, false, true); }
+    else { if (separable) GG_BLUR(3, true, false); else GG_BLUR(3, false, false); }
+  }
+  else if (mode == 1) {
     if (fast) { if (separable) GG_BLUR(1, true, true); else GG_BLUR(1, false, true); }
     else { if (separable) GG_BLUR(1, true, false); else GG_BLUR(1, false, false); }
   }
@@ -985,7 +1002,27 @@ int gg_blur_nhwc(void* out, void* out2, const void* in, const float* kernel, con
   GG_DISPATCH_T(dtype, "blur_nhwc",
                 return launch_blur<T_>(out, out2, in, kernel, noise, noise_weight, bias, row_scale, scale2, mul, row_dot,
                                        workspace, N, C, in_h, in_w, kernel_h, kernel_w, separable, pad_x0, pad_x1, pad_y0,
-                                       pad_y1, mode, act, alpha, scale, stream, dtype));
+                                       pad_y1, mode, act, alpha, scale, stream, dtype, false));
+  return GG_OK;
+}
+
+int gg_blur_nhwc_mask(void* mask, void* out2, const void* in, const float* kernel, const float* noise,
+                      const float* noise_weight, const float* bias, const float* row_scale, const float* scale2, int dtype,
+                      int64_t N, int C, int in_h, int in_w, int kernel_h, int kernel_w, int separable, int pad_x0, int pad_x1,
+                      int pad_y0, int pad_y1, int act, float alpha, float scale, void* stream) {
+  if (N < 0 || C < 0 || in_h < 1 || in_w < 1) return fail(GG_ERR_BAD_ARG, "blur_nhwc_mask: bad shape");
+  if (kernel_h < 1 || kernel_w < 1 || kernel_h > 4 || kernel_w > 4) return fail(GG_ERR_UNSUPPORTED, "blur_nhwc_mask: filter must be <= 4x4");
+  if (act != 1 && act != 3) return fail(GG_ERR_UNSUPPORTED, "blur_nhwc_mask: act must be 1 or 3");
+  if (dtype != GG_F32 && dtype != GG_BF16) return fail(GG_ERR_UNSUPPORTED, "blur_nhwc_mask: dtype %d not supported (fp32 or bf16)", dtype);
+  if (N == 0 || C == 0) return GG_OK;
+  if (!in || !kernel) return fail(GG_ERR_BAD_ARG, "blur_nhwc_mask: null tensor");
+  if (!mask) return fail(GG_ERR_BAD_ARG, "blur_nhwc_mask: null mask");
+  if (out2 && !scale2) return fail(GG_ERR_BAD_ARG, "blur_nhwc_mask: out2 needs scale2");
+  if (N > 65535) return fail(GG_ERR_UNSUPPORTED, "blur_nhwc_mask: batch > 65535");
+  GG_DISPATCH_T(dtype, "blur_nhwc_mask",
+                return launch_blur<T_>(mask, out2, in, kernel, noise, noise_weight, bias, row_scale, scale2, nullptr, nullptr,
+                                       nullptr, N, C, in_h, in_w, kernel_h, kernel_w, separable, pad_x0, pad_x1, pad_y0,
+                                       pad_y1, 1, act, alpha, scale, stream, dtype, true));
   return GG_OK;
 }
 

@@ -46,7 +46,8 @@ struct TailFwdParams {
 // the channel vectors v = lane + 8j: 4 independent 16-byte loads in flight per lane, every constant fetched once per 4 pixels.
 // FAST: the gain-folded epilogue max(T, T*slope) is valid for the launch (host check) -- compile-time, so that the general
 // select-and-scale epilogue is not predicated into the pixel loop next to it.
-template <typename T, bool FAST>
+// MASK: `out` is the sign mask (common.cuh) instead of the activation -- all a backward pass without reductions needs of o.
+template <typename T, bool FAST, bool MASK>
 __global__ void __launch_bounds__(kT, 2)
 styled_tail_nhwc_kernel(const TailFwdParams p) {
   constexpr int V = ChanVec<T>::V;
@@ -84,7 +85,8 @@ styled_tail_nhwc_kernel(const TailFwdParams p) {
   // multiplies and half the index registers (the bf16 instantiation sits at the 128-register cap of 2 CTAs/SM)
   const int hw = static_cast<int>(p.hw);
   const T* raw = static_cast<const T*>(p.raw) + n * hw * C;
-  T* out = p.out ? static_cast<T*>(p.out) + n * hw * C : nullptr;
+  T* out = (p.out && !MASK) ? static_cast<T*>(p.out) + n * hw * C : nullptr;
+  uint32_t* mask = MASK ? static_cast<uint32_t*>(p.out) + n * hw * (C >> 5) : nullptr;
   T* xs = p.xs ? static_cast<T*>(p.xs) + n * hw * C : nullptr;
   const float* noise_n = p.noise ? p.noise + n * hw : nullptr;
   const int q0 = static_cast<int>(p0), q1 = static_cast<int>(p1);
@@ -156,9 +158,15 @@ styled_tail_nhwc_kernel(const TailFwdParams p) {
             acc[u][2] = fmaf(w2[k], o[k], acc[u][2]);
           }
         }
+        uint32_t word = 0u;
+        if (MASK) word = sign_word<V>(sign_bits<T>(o), l, gmask);
         if (pb + u < q1) {
           const unsigned off = po[u] + static_cast<unsigned>(v * V);
-          if (out) stg_stream16(out + off, ChanVec<T>::pack(o));
+          if (MASK) {
+            if ((l * V & 31) == 0) mask[off >> 5] = word;
+          } else if (out) {
+            stg_stream16(out + off, ChanVec<T>::pack(o));
+          }
           if (xs) stg_stream16(xs + off, ChanVec<T>::pack(o2));
         }
       }
@@ -187,7 +195,7 @@ styled_tail_nhwc_kernel(const TailFwdParams p) {
 
 struct TailBwdParams {
   void* g_raw; float* partial;
-  const void* g_xs; const void* out; const void* raw;
+  const void* g_xs; const void* out; const void* raw;   // MASK: `out` is the forward pass's sign mask
   const float* s_next; const float* demod; const float* g_rgb; const float* wm;
   float alpha, gain;
   int C;
@@ -198,7 +206,8 @@ struct TailBwdParams {
 
 // Thread = (channel vector, pixel lane): a thread keeps its V channels for the whole chunk, so the per-channel sums live in
 // registers; they are combined across the CTA's pixel lanes through shared memory into one partial block per CTA.
-template <typename T>
+// MASK: lrelu' comes from the sign mask; nothing is reduced, so neither the activation nor `raw` is read.
+template <typename T, bool MASK>
 __global__ void __launch_bounds__(kT, 2)
 styled_tail_bwd_nhwc_kernel(const TailBwdParams p) {
   constexpr int V = ChanVec<T>::V;
@@ -215,6 +224,11 @@ styled_tail_bwd_nhwc_kernel(const TailBwdParams p) {
   for (int k = 0; k < V; ++k) a_ds[k] = a_dd[k] = a_g0[k] = a_g1[k] = a_g2[k] = 0.f;
   const T* gxs = static_cast<const T*>(p.g_xs);
   const T* outp = static_cast<const T*>(p.out);
+  const uint32_t* maskp = static_cast<const uint32_t*>(p.out) + n * p.hw * (C >> 5);     // this sample's words
+  const int mw = C >> 5;
+  auto load_out = [&](int64_t pu, int64_t off) {      // the activation vector, or (MASK) its V sign bits in .x
+    return MASK ? make_uint4(sign_load<V>(maskp + pu * mw, cq), 0u, 0u, 0u) : ldg_stream16(outp + off);
+  };
   const T* rawp = static_cast<const T*>(p.raw);
   T* graw = static_cast<T*>(p.g_raw);
   if (pl < lanes_p) {
@@ -233,19 +247,22 @@ styled_tail_bwd_nhwc_kernel(const TailBwdParams p) {
     auto body = [&](int64_t off, const uint4 gr, const uint4 orw, const uint4 rr, float s0, float s1, float s2) {
       float g[V], o[V], r[V], gt[V];
       ChanVec<T>::unpack(gr, g);
-      ChanVec<T>::unpack(orw, o);
+      if (!MASK) ChanVec<T>::unpack(orw, o);
       ChanVec<T>::unpack(rr, r);
 #pragma unroll
       for (int k = 0; k < V; ++k) {
         float go = g[k] * sv[k];
         if (p.g_rgb) go = fmaf(w2[k], s2, fmaf(w1[k], s1, fmaf(w0[k], s0, go)));
-        const float t = (o[k] > 0.f ? go : go * p.alpha) * p.gain;
-        a_ds[k] = fmaf(g[k], o[k], a_ds[k]);
-        a_dd[k] = fmaf(t, r[k], a_dd[k]);
-        a_g0[k] = fmaf(s0, o[k], a_g0[k]);
-        a_g1[k] = fmaf(s1, o[k], a_g1[k]);
-        a_g2[k] = fmaf(s2, o[k], a_g2[k]);
+        const bool pos = MASK ? ((orw.x >> k) & 1u) != 0u : o[k] > 0.f;
+        const float t = (pos ? go : go * p.alpha) * p.gain;
         gt[k] = t * dv[k];
+        if (!MASK) {
+          a_ds[k] = fmaf(g[k], o[k], a_ds[k]);
+          a_dd[k] = fmaf(t, r[k], a_dd[k]);
+          a_g0[k] = fmaf(s0, o[k], a_g0[k]);
+          a_g1[k] = fmaf(s1, o[k], a_g1[k]);
+          a_g2[k] = fmaf(s2, o[k], a_g2[k]);
+        }
       }
       *reinterpret_cast<uint4*>(graw + off) = ChanVec<T>::pack(gt);
     };
@@ -258,7 +275,7 @@ styled_tail_bwd_nhwc_kernel(const TailBwdParams p) {
       for (int u = 0; u < U; ++u) {
         const int64_t pu = pp + u * lanes_p;
         off[u] = ((n * p.hw + pu) * cv + cq) * V;
-        orw[u] = ldg_stream16(outp + off[u]);
+        orw[u] = load_out(pu, off[u]);
         gr[u] = gxs ? ldg_stream16(gxs + off[u]) : zero;
       }
 #pragma unroll
@@ -274,11 +291,11 @@ styled_tail_bwd_nhwc_kernel(const TailBwdParams p) {
     }
     for (; pp < p1; pp += lanes_p) {
       const int64_t off = ((n * p.hw + pp) * cv + cq) * V;
-      body(off, gxs ? ldg_stream16(gxs + off) : zero, ldg_stream16(outp + off), rawp ? ldg_stream16(rawp + off) : zero,
+      body(off, gxs ? ldg_stream16(gxs + off) : zero, load_out(pp, off), rawp ? ldg_stream16(rawp + off) : zero,
            g0 ? __ldg(g0 + pp) : 0.f, g0 ? __ldg(g0 + p.hw + pp) : 0.f, g0 ? __ldg(g0 + 2 * p.hw + pp) : 0.f);
     }
   }
-  if (p.partial && p.n_red > 0) {
+  if (!MASK && p.partial && p.n_red > 0) {
     const int R = p.n_red;
     if (pl < lanes_p) {
       float* row = red + static_cast<int64_t>(pl) * R * C + cq * V;
@@ -324,26 +341,26 @@ int64_t bwd_chunk(int64_t N, int cv, int64_t HW) {
 
 using namespace gg;
 
-extern "C" {
-
-int gg_styled_tail_nhwc(void* out, void* xs, float* rgb, const void* raw, const float* noise, const float* noise_weight,
-                        const float* bias, const float* demod, const float* s_next, const float* wm, const float* rgb_bias,
-                        const float* skip, int dtype, int act, float alpha, float scale, int64_t N, int C, int64_t HW,
-                        void* stream) {
-  if (N < 0 || C < 0 || HW < 0) return fail(GG_ERR_BAD_ARG, "styled_tail_nhwc: negative size");
-  if (dtype != GG_F32 && dtype != GG_BF16) return fail(GG_ERR_UNSUPPORTED, "styled_tail_nhwc: dtype %d not supported (fp32 or bf16)", dtype);
-  if (act != 1 && act != 3) return fail(GG_ERR_UNSUPPORTED, "styled_tail_nhwc: act must be 1 (linear) or 3 (lrelu)");
+// `out_is_mask`: `out` receives the sign mask (N, HW, C/32) uint32 instead of the activation.
+static int launch_tail_fwd(const char* who, void* out, bool out_is_mask, void* xs, float* rgb, const void* raw,
+                           const float* noise, const float* noise_weight, const float* bias, const float* demod,
+                           const float* s_next, const float* wm, const float* rgb_bias, const float* skip, int dtype, int act,
+                           float alpha, float scale, int64_t N, int C, int64_t HW, void* stream) {
+  if (N < 0 || C < 0 || HW < 0) return fail(GG_ERR_BAD_ARG, "%s: negative size", who);
+  if (dtype != GG_F32 && dtype != GG_BF16) return fail(GG_ERR_UNSUPPORTED, "%s: dtype %d not supported (fp32 or bf16)", who, dtype);
+  if (act != 1 && act != 3) return fail(GG_ERR_UNSUPPORTED, "%s: act must be 1 (linear) or 3 (lrelu)", who);
   if (N * HW * C == 0) return GG_OK;
   const int V = dtype == GG_BF16 ? 8 : 4;
-  if (C % (V * kGroup) != 0 || C > 2048) return fail(GG_ERR_UNSUPPORTED, "styled_tail_nhwc: C must be a multiple of %d, <= 2048", V * kGroup);
-  if (!raw || (!out && !xs && !rgb)) return fail(GG_ERR_BAD_ARG, "styled_tail_nhwc: null tensor");
-  if (xs && !s_next) return fail(GG_ERR_BAD_ARG, "styled_tail_nhwc: xs needs s_next");
-  if (rgb && !wm) return fail(GG_ERR_BAD_ARG, "styled_tail_nhwc: rgb needs wm");
+  if (C % (V * kGroup) != 0 || C > 2048) return fail(GG_ERR_UNSUPPORTED, "%s: C must be a multiple of %d, <= 2048", who, V * kGroup);
+  if (!raw || (!out && !xs && !rgb)) return fail(GG_ERR_BAD_ARG, "%s: null tensor", who);
+  if (out_is_mask && !out) return fail(GG_ERR_BAD_ARG, "%s: null mask", who);
+  if (xs && !s_next) return fail(GG_ERR_BAD_ARG, "%s: xs needs s_next", who);
+  if (rgb && !wm) return fail(GG_ERR_BAD_ARG, "%s: rgb needs wm", who);
   const int64_t chunk = fwd_chunk(N, HW);
-  if (chunk > 0x7fffff00LL || HW * C >= 0x7fffffffLL) return fail(GG_ERR_BAD_ARG, "styled_tail_nhwc: plane too large (H*W*C must be < 2^31)");
+  if (chunk > 0x7fffff00LL || HW * C >= 0x7fffffffLL) return fail(GG_ERR_BAD_ARG, "%s: plane too large (H*W*C must be < 2^31)", who);
   const int K = static_cast<int>((HW + chunk - 1) / chunk);
   const int64_t grid = N * K;
-  if (grid > 0x7fffffffLL) return fail(GG_ERR_BAD_ARG, "styled_tail_nhwc: too many CTAs");
+  if (grid > 0x7fffffffLL) return fail(GG_ERR_BAD_ARG, "%s: too many CTAs", who);
   TailFwdParams p;
   p.raw = raw; p.out = out; p.xs = xs; p.rgb = rgb; p.skip = rgb ? skip : nullptr;
   p.noise = noise; p.noise_weight = noise_weight; p.bias = bias; p.demod = demod; p.s_next = s_next;
@@ -353,15 +370,34 @@ int gg_styled_tail_nhwc(void* out, void* xs, float* rgb, const void* raw, const 
   auto st = static_cast<cudaStream_t>(stream);
   const bool fast = p.gain > 0.f && ((p.act == 3 && p.alpha >= 0.f && p.alpha <= 1.f) || p.act == 1);
   const unsigned g = static_cast<unsigned>(grid);
-  if (dtype == GG_F32) {
-    if (fast) styled_tail_nhwc_kernel<float, true><<<g, kT, smem, st>>>(p);
-    else styled_tail_nhwc_kernel<float, false><<<g, kT, smem, st>>>(p);
-  } else {
-    if (fast) styled_tail_nhwc_kernel<__nv_bfloat16, true><<<g, kT, smem, st>>>(p);
-    else styled_tail_nhwc_kernel<__nv_bfloat16, false><<<g, kT, smem, st>>>(p);
-  }
+#define GG_TAIL(T_, F_)                                                                   \
+  do {                                                                                    \
+    if (out_is_mask) styled_tail_nhwc_kernel<T_, F_, true><<<g, kT, smem, st>>>(p);       \
+    else styled_tail_nhwc_kernel<T_, F_, false><<<g, kT, smem, st>>>(p);                  \
+  } while (0)
+  if (dtype == GG_F32) { if (fast) GG_TAIL(float, true); else GG_TAIL(float, false); }
+  else { if (fast) GG_TAIL(__nv_bfloat16, true); else GG_TAIL(__nv_bfloat16, false); }
+#undef GG_TAIL
   GG_CHECK_LAUNCH("styled_tail_nhwc launch");
   return GG_OK;
+}
+
+extern "C" {
+
+int gg_styled_tail_nhwc(void* out, void* xs, float* rgb, const void* raw, const float* noise, const float* noise_weight,
+                        const float* bias, const float* demod, const float* s_next, const float* wm, const float* rgb_bias,
+                        const float* skip, int dtype, int act, float alpha, float scale, int64_t N, int C, int64_t HW,
+                        void* stream) {
+  return launch_tail_fwd("styled_tail_nhwc", out, false, xs, rgb, raw, noise, noise_weight, bias, demod, s_next, wm, rgb_bias,
+                         skip, dtype, act, alpha, scale, N, C, HW, stream);
+}
+
+int gg_styled_tail_mask_nhwc(void* mask, void* xs, float* rgb, const void* raw, const float* noise, const float* noise_weight,
+                             const float* bias, const float* demod, const float* s_next, const float* wm,
+                             const float* rgb_bias, const float* skip, int dtype, int act, float alpha, float scale, int64_t N,
+                             int C, int64_t HW, void* stream) {
+  return launch_tail_fwd("styled_tail_mask_nhwc", mask, true, xs, rgb, raw, noise, noise_weight, bias, demod, s_next, wm,
+                         rgb_bias, skip, dtype, act, alpha, scale, N, C, HW, stream);
 }
 
 int64_t gg_styled_tail_backward_workspace(int dtype, int64_t N, int C, int64_t HW) {
@@ -410,16 +446,16 @@ int gg_styled_tail_backward_nhwc(void* g_raw, float* d_s_next, float* d_demod, f
   if (smem > 48 * 1024) {
     static DeviceOnce configured;
     if (configured.needed()) {
-      cudaError_t e = cudaFuncSetAttribute(styled_tail_bwd_nhwc_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
+      cudaError_t e = cudaFuncSetAttribute(styled_tail_bwd_nhwc_kernel<float, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
       if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(styled_tail_bwd_nhwc_kernel<__nv_bfloat16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
+        e = cudaFuncSetAttribute(styled_tail_bwd_nhwc_kernel<__nv_bfloat16, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
       if (e != cudaSuccess) return cuda_fail(e, "styled_tail_backward_nhwc smem opt-in");
       configured.done();
     }
     if (smem > 100 * 1024) return fail(GG_ERR_UNSUPPORTED, "styled_tail_backward_nhwc: C too large for the reduction stage");
   }
-  if (dtype == GG_F32) styled_tail_bwd_nhwc_kernel<float><<<static_cast<unsigned>(grid), kT, smem, st>>>(p);
-  else styled_tail_bwd_nhwc_kernel<__nv_bfloat16><<<static_cast<unsigned>(grid), kT, smem, st>>>(p);
+  if (dtype == GG_F32) styled_tail_bwd_nhwc_kernel<float, false><<<static_cast<unsigned>(grid), kT, smem, st>>>(p);
+  else styled_tail_bwd_nhwc_kernel<__nv_bfloat16, false><<<static_cast<unsigned>(grid), kT, smem, st>>>(p);
   GG_CHECK_LAUNCH("styled_tail_backward_nhwc launch");
   if (r > 0) {
     // partial is [N][K][r*C]: ONE finish launch writes every requested sum.  The caller's destinations are slices of one
@@ -444,6 +480,33 @@ int gg_styled_tail_backward_nhwc(void* g_raw, float* d_s_next, float* d_demod, f
     }
     GG_CHECK_LAUNCH("styled_tail_backward_nhwc finish launch");
   }
+  return GG_OK;
+}
+
+int gg_styled_tail_backward_mask_nhwc(void* g_raw, const void* g_xs, const float* g_rgb, const void* mask,
+                                      const float* s_next, const float* demod, const float* wm, int dtype, float alpha,
+                                      float scale, int64_t N, int C, int64_t HW, void* stream) {
+  if (N < 0 || C < 0 || HW < 0) return fail(GG_ERR_BAD_ARG, "styled_tail_backward_mask_nhwc: negative size");
+  if (dtype != GG_F32 && dtype != GG_BF16) return fail(GG_ERR_UNSUPPORTED, "styled_tail_backward_mask_nhwc: dtype %d not supported", dtype);
+  if (N * HW * C == 0) return GG_OK;
+  const int V = dtype == GG_BF16 ? 8 : 4;
+  if (C % 32 != 0 || C / V > kT) return fail(GG_ERR_UNSUPPORTED, "styled_tail_backward_mask_nhwc: C must be a multiple of 32, <= %d", V * kT);
+  if (!g_raw || !mask || (!g_xs && !g_rgb)) return fail(GG_ERR_BAD_ARG, "styled_tail_backward_mask_nhwc: null tensor");
+  if (g_xs && !s_next) return fail(GG_ERR_BAD_ARG, "styled_tail_backward_mask_nhwc: g_xs needs s_next");
+  if (g_rgb && !wm) return fail(GG_ERR_BAD_ARG, "styled_tail_backward_mask_nhwc: g_rgb needs wm");
+  const int64_t chunk64 = bwd_chunk(N, C / V, HW);
+  if (chunk64 > 0x7fffffffLL) return fail(GG_ERR_BAD_ARG, "styled_tail_backward_mask_nhwc: plane too large");
+  const int K = static_cast<int>((HW + chunk64 - 1) / chunk64);
+  const int64_t grid = N * K;
+  if (grid > 0x7fffffffLL) return fail(GG_ERR_BAD_ARG, "styled_tail_backward_mask_nhwc: too many CTAs");
+  TailBwdParams p;
+  p.g_raw = g_raw; p.partial = nullptr; p.g_xs = g_xs; p.out = mask; p.raw = nullptr; p.s_next = s_next; p.demod = demod;
+  p.g_rgb = g_rgb; p.wm = wm; p.alpha = alpha; p.gain = scale; p.C = C; p.hw = HW; p.chunk = static_cast<int>(chunk64);
+  p.chunks_per_sample = K; p.r_ds = p.r_dd = p.r_gw = -1; p.n_red = 0;
+  auto st = static_cast<cudaStream_t>(stream);
+  if (dtype == GG_F32) styled_tail_bwd_nhwc_kernel<float, true><<<static_cast<unsigned>(grid), kT, 0, st>>>(p);
+  else styled_tail_bwd_nhwc_kernel<__nv_bfloat16, true><<<static_cast<unsigned>(grid), kT, 0, st>>>(p);
+  GG_CHECK_LAUNCH("styled_tail_backward_mask_nhwc launch");
   return GG_OK;
 }
 

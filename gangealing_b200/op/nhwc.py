@@ -55,9 +55,17 @@ def noise_plane(noise, n, h, w):
     return noise.float().contiguous()
 
 
+def sign_mask_empty(n, c, h, w, device):
+    """Storage of the sign mask of an (N, C, H, W) channels-last activation: (N, H, W, C/32) 32-bit words (csrc/common.cuh)."""
+    if c % 32:
+        raise RuntimeError("sign mask: C = %d is not a multiple of 32" % c)
+    return torch.empty((n, h, w, c // 32), dtype=torch.int32, device=device)
+
+
 def blur(x, kernel, pad, mode=0, noise=None, noise_weight=None, bias=None, row_scale=None, scale2=None, want_out=True,
-         want_out2=False, mul=None, want_dot=False, negative_slope=0.2, gain=1.0, act=3):
-    """gg_blur_nhwc.  pad = (x0, x1, y0, y1).  -> (out, out2, row_dot)."""
+         want_out2=False, mul=None, want_dot=False, negative_slope=0.2, gain=1.0, act=3, want_mask=False):
+    """gg_blur_nhwc.  pad = (x0, x1, y0, y1).  -> (out, out2, row_dot).  want_mask (mode 1): gg_blur_nhwc_mask, `out` is the
+    sign mask of the activation instead of the activation."""
     n, c, in_h, in_w = x.shape
     taps = kernel.detach()
     if taps.dtype != torch.float32 or not taps.is_contiguous():
@@ -72,7 +80,12 @@ def blur(x, kernel, pad, mode=0, noise=None, noise_weight=None, bias=None, row_s
 
     def empty():
         return torch.empty((n, c, out_h, out_w), dtype=x.dtype, device=x.device, memory_format=CL)
-    out = empty() if (want_out or mode != 1) else None
+    if want_mask and mode != 1:
+        raise RuntimeError("blur: the sign mask belongs to the fused tail (mode 1)")
+    if want_mask:
+        out = sign_mask_empty(n, c, out_h, out_w, x.device)
+    else:
+        out = empty() if (want_out or mode != 1) else None
     out2 = empty() if (mode == 1 and want_out2) else None
     nz = noise_plane(noise, n, out_h, out_w) if mode == 1 else None
     dot = ws = None
@@ -89,17 +102,24 @@ def blur(x, kernel, pad, mode=0, noise=None, noise_weight=None, bias=None, row_s
         ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         ev0.record()
     nw, b, rs, s2 = _f32(noise_weight, 1), _f32(bias, c), _f32(row_scale, n * c), _f32(scale2, n * c)
-    rc = lib.gg_blur_nhwc(_lib.ptr(out), _lib.ptr(out2), x.data_ptr(), taps.data_ptr(), _lib.ptr(nz),
-                          _lib.ptr(nw), _lib.ptr(b), _lib.ptr(rs),
-                          _lib.ptr(s2), _lib.ptr(mul if dot is not None else None), _lib.ptr(dot), _lib.ptr(ws),
-                          code, n, c, in_h, in_w, kh, kw, 1 if _lib.filter_is_separable(kernel) else 0, pad[0], pad[1],
-                          pad[2], pad[3], mode, act, negative_slope, gain, _lib.stream())
-    _lib.check(rc, "gg_blur_nhwc")
+    sep = 1 if _lib.filter_is_separable(kernel) else 0
+    if want_mask:
+        rc = lib.gg_blur_nhwc_mask(out.data_ptr(), _lib.ptr(out2), x.data_ptr(), taps.data_ptr(), _lib.ptr(nz), _lib.ptr(nw),
+                                   _lib.ptr(b), _lib.ptr(rs), _lib.ptr(s2), code, n, c, in_h, in_w, kh, kw, sep, pad[0],
+                                   pad[1], pad[2], pad[3], act, negative_slope, gain, _lib.stream())
+    else:
+        rc = lib.gg_blur_nhwc(_lib.ptr(out), _lib.ptr(out2), x.data_ptr(), taps.data_ptr(), _lib.ptr(nz),
+                              _lib.ptr(nw), _lib.ptr(b), _lib.ptr(rs),
+                              _lib.ptr(s2), _lib.ptr(mul if dot is not None else None), _lib.ptr(dot), _lib.ptr(ws),
+                              code, n, c, in_h, in_w, kh, kw, sep, pad[0], pad[1],
+                              pad[2], pad[3], mode, act, negative_slope, gain, _lib.stream())
+    _lib.check(rc, "gg_blur_nhwc_mask" if want_mask else "gg_blur_nhwc")
     if timed:
         ev1.record()
         es = x.element_size()
-        writes = (out is not None) + (out2 is not None)
+        writes = (out is not None and not want_mask) + (out2 is not None)
         TIMING.append((ev0, ev1, es * n * c * (in_h * in_w + writes * out_h * out_w) + (4 * n * out_h * out_w if nz is not None else 0)
+                       + (out.numel() * 4 if want_mask else 0)
                        + 4 * ((2 + (scale2 is not None)) * c + 1 + kh * kw)))
     return out, out2, dot
 
@@ -144,10 +164,15 @@ def channel_scale(x, s, y=None):
     return out, dot
 
 
-def styled_tail(raw, noise, noise_weight, bias, demod, s_next, wm, rgb_bias, skip, want_out, negative_slope, gain, act=3):
-    """gg_styled_tail_nhwc -> (out or None, xs or None, rgb or None)."""
+def styled_tail(raw, noise, noise_weight, bias, demod, s_next, wm, rgb_bias, skip, want_out, negative_slope, gain, act=3,
+                want_mask=False):
+    """gg_styled_tail_nhwc -> (out or None, xs or None, rgb or None).  want_mask: gg_styled_tail_mask_nhwc, the first
+    result is the sign mask of the activation instead of the activation."""
     n, c, h, w = raw.shape
-    out = torch.empty_like(raw) if want_out else None
+    if want_mask:
+        out = sign_mask_empty(n, c, h, w, raw.device)
+    else:
+        out = torch.empty_like(raw) if want_out else None
     xs = torch.empty_like(raw) if s_next is not None else None
     rgb = torch.empty((n, 3, h, w), dtype=torch.float32, device=raw.device) if wm is not None else None
     sk = None
@@ -159,10 +184,11 @@ def styled_tail(raw, noise, noise_weight, bias, demod, s_next, wm, rgb_bias, ski
             raise RuntimeError("styled_tail: skip must be (N, 3, H, W)")
     consts = [noise_plane(noise, n, h, w), _f32(noise_weight, 1), _f32(bias, c), _f32(demod, n * c), _f32(s_next, n * c),
               _f32(wm, n * 3 * c), _f32(rgb_bias, 3)]
-    rc = _lib.load().gg_styled_tail_nhwc(_lib.ptr(out), _lib.ptr(xs), _lib.ptr(rgb), raw.data_ptr(),
-                                         *[_lib.ptr(t) for t in consts], _lib.ptr(sk),
-                                         _lib.dtype_code(raw), act, negative_slope, gain, n, c, h * w, _lib.stream())
-    _lib.check(rc, "gg_styled_tail_nhwc")
+    lib = _lib.load()
+    entry = lib.gg_styled_tail_mask_nhwc if want_mask else lib.gg_styled_tail_nhwc
+    rc = entry(_lib.ptr(out), _lib.ptr(xs), _lib.ptr(rgb), raw.data_ptr(), *[_lib.ptr(t) for t in consts], _lib.ptr(sk),
+               _lib.dtype_code(raw), act, negative_slope, gain, n, c, h * w, _lib.stream())
+    _lib.check(rc, "gg_styled_tail_mask_nhwc" if want_mask else "gg_styled_tail_nhwc")
     return out, xs, rgb
 
 
@@ -198,3 +224,23 @@ def styled_tail_backward(g_xs, g_rgb, out_saved, raw, s_next, demod, wm, want_ds
                                           code, negative_slope, gain, n, c, h * w, rows * c, _lib.stream())
     _lib.check(rc, "gg_styled_tail_backward_nhwc")
     return g_raw, d_s, d_d, d_w
+
+
+def styled_tail_backward_mask(g_xs, g_rgb, mask, s_next, demod, wm, negative_slope, gain, dtype):
+    """gg_styled_tail_backward_mask_nhwc -> g_raw (channels-last (N, C, H, W) of `dtype`): the data gradient of the tail
+    from the forward pass's sign mask (N, H, W, C/32), when no style, demodulation or to-RGB weight gradient is wanted."""
+    n, h, w, words = mask.shape
+    c = 32 * words
+    g_raw = torch.empty((n, c, h, w), dtype=dtype, device=mask.device, memory_format=CL)
+    if g_xs is not None and (g_xs.shape != g_raw.shape or g_xs.dtype != dtype or not g_xs.is_contiguous(memory_format=CL)
+                             or not _lib.aligned16(g_xs)):
+        raise RuntimeError("styled_tail_backward_mask: g_xs must be a 16-byte-aligned channels-last tensor of the "
+                               "activation's shape and dtype")
+    if g_rgb is not None and (g_rgb.shape != (n, 3, h, w) or g_rgb.dtype != torch.float32 or not g_rgb.is_contiguous()):
+        raise RuntimeError("styled_tail_backward_mask: g_rgb must be a dense fp32 (N, 3, H, W) tensor")
+    consts = [_f32(s_next, n * c), _f32(demod, n * c), _f32(wm, n * 3 * c)]
+    rc = _lib.load().gg_styled_tail_backward_mask_nhwc(g_raw.data_ptr(), _lib.ptr(g_xs), _lib.ptr(g_rgb), mask.data_ptr(),
+                                                       *[_lib.ptr(t) for t in consts], _lib.dtype_code(g_raw),
+                                                       negative_slope, gain, n, c, h * w, _lib.stream())
+    _lib.check(rc, "gg_styled_tail_backward_mask_nhwc")
+    return g_raw

@@ -33,7 +33,7 @@ class _Plan:
             w = torch.stack([(lin.weight.detach() * lin.scale).t().contiguous() for _, lin, _ in members])     # (L, D, C)
             b = torch.stack([(lin.bias.detach() * lin.lr_mul) for _, lin, _ in members]).unsqueeze(1)          # (L, 1, C)
             idx = torch.tensor([li for _, _, li in members], device=w.device)
-            self.groups.append((w, b, idx, [key for key, _, _ in members]))
+            self.groups.append((w, b, idx, [key for key, _, _ in members], [li for _, _, li in members]))
         self.stamp = tuple((lin.weight._version, lin.weight.data_ptr(), lin.bias._version) for _, lin, _ in mods)
 
     def valid(self, convs, rgbs):
@@ -41,18 +41,21 @@ class _Plan:
         return self.stamp == tuple((lin.weight._version, lin.weight.data_ptr(), lin.bias._version) for lin in mods)
 
 
-def all_styles(generator, latent, convs, rgbs, conv_idx, rgb_idx):
-    """-> (styles of the StyledConvs, styles of the ToRGBs): lists of (B, C_in) fp32 tensors, differentiable in `latent`."""
+def all_styles(generator, latent, convs, rgbs, conv_idx, rgb_idx, row_needs_grad=None):
+    """-> (styles of the StyledConvs, styles of the ToRGBs): lists of (B, C_in) fp32 tensors, differentiable in `latent`.
+    row_needs_grad: per latent row, whether what the caller built that row from requires grad (None: as `latent` does).  A
+    style read from a constant row is returned detached: the values are those of the same batched GEMM, but its consumers
+    (demodulation, the fused tails) then see that nothing is owed to it and skip that part of their backward."""
     plan = getattr(generator, "_gg_style_plan", None)
     if plan is None or not plan.valid(convs, rgbs):
         plan = _Plan(convs, rgbs, conv_idx, rgb_idx)
         generator._gg_style_plan = plan
     out = {}
-    for w, b, idx, keys in plan.groups:
+    for w, b, idx, keys, rows in plan.groups:
         lat = latent.index_select(1, idx).transpose(0, 1)          # (L, B, D)
         s = torch.baddbmm(b, lat, w)                               # (L, B, C)
         for j, key in enumerate(keys):
-            out[key] = s[j]
+            out[key] = s[j] if row_needs_grad is None or row_needs_grad[rows[j]] else s[j].detach()
     return [out[("conv", i)] for i in range(len(convs))], [out[("rgb", i)] for i in range(len(rgbs))]
 
 
@@ -81,6 +84,8 @@ class _DemodAll(Function):
                                           I(*[w.shape[1] for w in weights]), I(*[w.shape[2] for w in weights]), float(eps), b,
                                           _lib.stream())
         _lib.check(rc, "gg_modconv_demod_batched")
+        # a coefficient whose style is constant is constant: its consumers owe it no gradient
+        ctx.mark_non_differentiable(*[o for l, o in enumerate(outs) if not ctx.needs_input_grad[1 + l]])
         ctx.save_for_backward(*ss, *outs, *wsqs)
         ctx.cfg = (n, tuple(float(x) for x in scales), tuple(s.dtype for s in styles))
         return tuple(outs)

@@ -8,9 +8,11 @@ to-RGB 1x1 grouped convolution + bias + up-sampled skip.  Here, per layer:
     xs', rgb = fused_tail(raw, ...)             ONE kernel: [blur +] demodulation + noise + bias + lrelu, emits the NEXT
                                                 convolution's modulated input xs' = o * s_next and (conv layers) the
                                                 to-RGB image rgb = wm . o + bias + skip -- the unscaled activation o is
-                                                written only when a backward pass will need it
+                                                written only when a backward pass will reduce over it
 and the backward of a fused tail is one pass (two for the blur layers), with the style / demodulation / to-RGB weight
-gradients reduced inside it (csrc/styled.cu, csrc/nhwc.cu mode 2).  Round 1's separate `channel_scale` passes (15.7 % of
+gradients reduced inside it (csrc/styled.cu, csrc/nhwc.cu mode 2).  A layer whose styles are constants (every layer above
+the latent learner's inject index) owes the backward pass only g_raw, and g_raw needs only the SIGN of o: such a tail writes
+a sign mask (1 bit per element) instead of o and keeps neither o nor raw; its backward reads (g_xs, mask).  Round 1's separate `channel_scale` passes (15.7 % of
 the step), the to-RGB kernels, the gradient add of the RGB branch and the demodulation row-dot pass are gone.
 
 Only the frozen-generator case GANgealing needs is fused (gradients flow to the latents/styles, never to the generator's
@@ -35,21 +37,24 @@ class _FusedTail(Function):
     def forward(ctx, raw, demod, s_next, wm, skip, noise, noise_weight, bias, rgb_bias, kernel, pad, negative_slope, gain):
         _lib.require_cuda(raw, demod, s_next, wm, skip, noise)
         needs = ctx.needs_input_grad
-        save = needs[0] or needs[1] or needs[2] or needs[3]
+        reduces = needs[1] or needs[2] or needs[3]      # a sum over the activation is owed to demod, s_next or wm
+        save = needs[0] or reduces
+        # only g_raw is owed: the backward pass needs lrelu'(o), the sign mask, and neither o nor raw
+        masked = needs[0] and not reduces and (kernel is None or s_next is not None)
         if kernel is None:
-            out, xs, rgb = nhwc.styled_tail(raw, noise, noise_weight, bias, demod, s_next, wm, rgb_bias, skip, save,
-                                            negative_slope, gain)
+            out, xs, rgb = nhwc.styled_tail(raw, noise, noise_weight, bias, demod, s_next, wm, rgb_bias, skip,
+                                            save and not masked, negative_slope, gain, want_mask=masked)
         else:
             if wm is not None:
                 raise RuntimeError("fused tail: the blur (up-sampling) layers carry no to-RGB branch")
             pad4 = (pad[0], pad[1], pad[0], pad[1])
             out, xs, _ = nhwc.blur(raw, kernel, pad4, mode=1, noise=noise, noise_weight=noise_weight, bias=bias,
-                                   row_scale=demod, scale2=s_next, want_out=save or s_next is None,
-                                   want_out2=s_next is not None, negative_slope=negative_slope, gain=gain)
+                                   row_scale=demod, scale2=s_next, want_out=(save and not masked) or s_next is None,
+                                   want_out2=s_next is not None, negative_slope=negative_slope, gain=gain, want_mask=masked)
             rgb = None
-        ctx.cfg = (kernel is not None, pad, negative_slope, gain, tuple(raw.shape))
+        ctx.cfg = (kernel is not None, pad, negative_slope, gain, tuple(raw.shape), masked, raw.dtype)
         if save:
-            ctx.save_for_backward(raw if (needs[1] and demod is not None) else None, out,
+            ctx.save_for_backward(raw if (needs[1] and demod is not None) else None, out,      # masked: `out` is the mask
                                   demod.detach() if demod is not None else None,
                                   s_next.detach() if s_next is not None else None,
                                   wm.detach() if wm is not None else None, kernel)
@@ -61,28 +66,33 @@ class _FusedTail(Function):
     @once_differentiable
     def backward(ctx, g_xs, g_rgb):
         raw, out, demod, s_next, wm, kernel = ctx.saved_tensors
-        is_blur, pad, negative_slope, gain, raw_shape = ctx.cfg
+        is_blur, pad, negative_slope, gain, raw_shape, masked, dtype = ctx.cfg
         need_raw, need_d, need_s, need_w, need_skip = ctx.needs_input_grad[:5]
         if g_xs is not None:
             g_xs = g_xs.contiguous(memory_format=CL)
-            if g_xs.dtype != out.dtype:
-                g_xs = g_xs.to(out.dtype)
+            if g_xs.dtype != dtype:
+                g_xs = g_xs.to(dtype)
         if g_rgb is not None:
             g_rgb = g_rgb.float().contiguous()
         g_raw = d_s = d_d = d_w = None
         if g_xs is None and g_rgb is None:
             return (None,) * 13
-        if not is_blur:
+        if masked and not is_blur:
+            g_raw = nhwc.styled_tail_backward_mask(g_xs, g_rgb, out, s_next, demod, wm, negative_slope, gain, dtype)
+        elif not is_blur:
             g_raw, d_s, d_d, d_w = nhwc.styled_tail_backward(
                 g_xs, g_rgb, out, raw, s_next, demod, wm, need_s, need_d and demod is not None, need_w,
                 negative_slope, gain)
         else:
             # pass 1: g_t = lrelu'(out)*gain*(g_xs*s_next)   (+ d_s_next)      pass 2: adjoint blur, *demod, <B^T g_t, raw>
-            g_t, d_s, _, _ = nhwc.styled_tail_backward(g_xs, None, out, None, s_next, None, None, need_s, False, False,
-                                                       negative_slope, gain)
+            if masked:
+                g_t = nhwc.styled_tail_backward_mask(g_xs, None, out, s_next, None, None, negative_slope, gain, dtype)
+            else:
+                g_t, d_s, _, _ = nhwc.styled_tail_backward(g_xs, None, out, None, s_next, None, None, need_s, False, False,
+                                                           negative_slope, gain)
             kh, kw = kernel.shape
             pad4 = (pad[0], pad[1], pad[0], pad[1])
-            gp = grad_pad(raw_shape[2], raw_shape[3], out.shape[2], out.shape[3], kh, kw, (1, 1), (1, 1), pad4)
+            gp = grad_pad(raw_shape[2], raw_shape[3], g_t.shape[2], g_t.shape[3], kh, kw, (1, 1), (1, 1), pad4)
             want_dot = need_d and demod is not None
             g_raw, _, d_d = nhwc.blur(g_t, _lib.flipped_filter(kernel), gp, mode=2, row_scale=demod, mul=raw if want_dot else None,
                                       want_dot=want_dot)
@@ -119,15 +129,16 @@ def fusable(generator, latent, act_dtype):
     return not any(p.requires_grad for p in generator.parameters())
 
 
-def synthesis(generator, latent, noise, act_dtype=torch.float32):
+def synthesis(generator, latent, noise, act_dtype=torch.float32, row_needs_grad=None):
     """Generator.forward's synthesis network (reference networks.py:562-586) on the fused path.  latent: (B, n_latent, D);
-    noise: list (one entry per StyledConv; None entries are sampled, in the reference's order).  -> image (B, 3, S, S) fp32."""
+    noise: list (one entry per StyledConv; None entries are sampled, in the reference's order); row_needs_grad: see
+    style_path.all_styles.  -> image (B, 3, S, S) fp32."""
     layers = [generator.conv1] + list(generator.convs)
     rgbs = [generator.to_rgb1] + list(generator.to_rgbs)
     b = latent.shape[0]
     # the whole style path up front, batched over layers (op/style_path.py): 3 GEMMs + 1 wgmma launch instead of 33 chains
     styles, rgb_styles = style_path.all_styles(generator, latent, layers, rgbs, list(range(len(layers))),
-                                               [2 * r + 1 for r in range(len(rgbs))])
+                                               [2 * r + 1 for r in range(len(rgbs))], row_needs_grad)
     demods = style_path.all_demod([layer.conv.weight for layer in layers], styles, [layer.conv.scale for layer in layers],
                                   layers[0].conv.eps)
     x0 = generator.input(latent).to(act_dtype).contiguous(memory_format=CL)

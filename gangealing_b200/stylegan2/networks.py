@@ -420,6 +420,7 @@ class Generator(nn.Module):
                 [getattr(self.noises, f"noise_{i}") for i in range(self.num_layers)]
         if truncation < 1:
             styles = [truncation_latent + truncation * (styles[0] - truncation_latent), styles[0]]
+        row_needs_grad = None       # per latent row; None: whatever `latent` itself says
         if len(styles) < 2 or inject_index == self.n_latent:
             inject_index = self.n_latent
             latent = styles[0].unsqueeze(1).repeat(1, inject_index, 1) if styles[0].ndim < 3 else styles[0]
@@ -428,11 +429,13 @@ class Generator(nn.Module):
                 inject_index = random.randint(1, self.n_latent - 1)
             latent = torch.cat([styles[0].unsqueeze(1).repeat(1, inject_index, 1),
                                 styles[1].unsqueeze(1).repeat(1, self.n_latent - inject_index, 1)], 1)
+            # the concatenation requires grad as soon as one part does; the fused synthesis is told which rows really do
+            row_needs_grad = [styles[0].requires_grad] * inject_index + [styles[1].requires_grad] * (self.n_latent - inject_index)
 
         if self.channels_last and self.fuse_synthesis and self.ops_are_native():
             from ..op import styled_fused
             if styled_fused.fusable(self, latent, self.act_dtype):
-                image = styled_fused.synthesis(self, latent, noise, self.act_dtype)
+                image = styled_fused.synthesis(self, latent, noise, self.act_dtype, row_needs_grad)
                 return (image, latent) if return_latents else (image, None)
         x0 = self.input(latent)
         if self.channels_last:

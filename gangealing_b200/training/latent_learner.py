@@ -108,18 +108,25 @@ class DirectionInterpolator(nn.Module):
         self.coefficients = nn.Parameter(initializer.detach().clone())
         self.n_latent, self.inject_index, self.num_heads = n_latent, inject_index, num_heads
 
-    def forward(self, styled_latent, psi=None, lat_mean=None, pca=None, unfold=False):
+    def forward(self, styled_latent, psi=None, lat_mean=None, pca=None, unfold=False, split=False):
         if pca is not None:
             return self.assign_buffers(pca)
-        return self.interpolate(styled_latent, psi, lat_mean, unfold)
+        return self.interpolate(styled_latent, psi, lat_mean, unfold, split)
 
-    def interpolate(self, styled_latent, psi, lat_mean=None, unfold=False):
+    def interpolate(self, styled_latent, psi, lat_mean=None, unfold=False, split=False):
+        """-> [(N*K, n_latent, D)], the reference's return value.  split=True: the same latent as the generator's two-latent
+        form [(N*K, D) truncated, (N*K, D) fixed] for `inject_index=self.inject_index`: the generator then sees that the
+        rows from the inject index up are constants (only `truncated` depends on the coefficients)."""
         assert len(styled_latent) == 1
         w = styled_latent[0]
         n = w.size(0)
         mean = self.lat_mean if lat_mean is None else lat_mean
         target = (mean + self.coefficients @ self.directions).repeat(n, 1)          # (N*K, D)
         w = w.repeat_interleave(self.num_heads, dim=0)
+        if split:
+            if unfold:
+                raise ValueError("DirectionInterpolator: unfold and split are exclusive")
+            return [target.lerp(w, psi), w]
         truncated = target.lerp(w, psi).unsqueeze(1).repeat(1, self.inject_index, 1)
         fixed = w.unsqueeze(1).repeat(1, self.n_latent - self.inject_index, 1)
         out = torch.cat([truncated, fixed], dim=1)

@@ -15,8 +15,10 @@ def sample_gan_supervised_pairs(generator, ll, resize_fake2stn, psi, batch, dim_
         if z is None:
             z = torch.randn(batch, dim_latent, device=device)
         unaligned_in, w_noise = generator([z], noise=None, return_latents=True)
-        w_aligned = ll([w_noise[:, 0, :]], psi=psi)
-        aligned_target, _ = generator(w_aligned, input_is_latent=True, noise=None)
+        # the latent learner's output in the generator's two-latent form: the rows above the inject index are w itself
+        w_aligned = ll([w_noise[:, 0, :]], psi=psi, split=True)
+        inject = getattr(ll, "module", ll).inject_index
+        aligned_target, _ = generator(w_aligned, input_is_latent=True, inject_index=inject, noise=None)
         aligned_target = resize_fake2stn(aligned_target)
     return unaligned_in, aligned_target
 

@@ -291,6 +291,9 @@ GG_API int gg_modconv_modulate(float* out, const float* weight, const float* sty
  *          input with its style modulation applied (networks.py:236,243), written by the pass that produces o
  *       2  adjoint epilogue (backward of mode 1's blur): t = B(in); out = t*row_scale[n,c]; row_dot[n,c] = sum_yx t*mul[n,y,x,c]
  *          (mul: same shape as out; NULL row_dot: no reduction) -- `workspace` of gg_blur_nhwc_workspace() bytes
+ *   gg_blur_nhwc_mask: mode 1 with the SIGN MASK of o in place of `out`: mask[n,y,x,w] bit b = (o[n,y,x,32w+b] > 0, tested
+ *     on the value as stored in `dtype`), (N, H, W, C/32) uint32 -- what the activation's derivative (op/fused_act.py:20-38)
+ *     needs of o when nothing is reduced over it (gg_styled_tail_backward_mask_nhwc).  out2 as in mode 1 (may be NULL).
  *   workspaces: gg_nhwc_rowwise_workspace(N, C, HW) bytes for the optional reductions (row_dot (N, C); grad_bias (C)).
  * ---------------------------------------------------------------------------------------------- */
 GG_API int gg_noise_bias_act_nhwc(void* out, const void* x, const float* noise, const float* noise_weight,
@@ -309,6 +312,11 @@ GG_API int gg_blur_nhwc(void* out, void* out2, const void* in, const float* kern
                         const void* mul, float* row_dot, void* workspace, int dtype, int64_t N, int C, int in_h,
                         int in_w, int kernel_h, int kernel_w, int separable, int pad_x0, int pad_x1, int pad_y0,
                         int pad_y1, int mode, int act, float alpha, float scale, void* stream);
+GG_API int gg_blur_nhwc_mask(void* mask, void* out2, const void* in, const float* kernel, const float* noise,
+                             const float* noise_weight, const float* bias, const float* row_scale, const float* scale2,
+                             int dtype, int64_t N, int C, int in_h, int in_w, int kernel_h, int kernel_w, int separable,
+                             int pad_x0, int pad_x1, int pad_y0, int pad_y1, int act, float alpha, float scale,
+                             void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * StyledConv / ToRGB tails fused across layer boundaries (csrc/styled.cu), channels-last, dtype as above.
@@ -328,6 +336,10 @@ GG_API int gg_blur_nhwc(void* out, void* out2, const void* in, const float* kern
  *      reduce_pitch: floats between consecutive samples of the sum outputs -- C (each a dense (N, C) / (N, 3, C) tensor) or
  *      R*C when they are the row slices [d_s_next | d_demod | d_wm x3] (requested ones only, in that order) of ONE (N, R, C)
  *      block, which is then finished by a single launch.
+ *   gg_styled_tail_mask_nhwc: gg_styled_tail_nhwc with the sign mask of o (see gg_blur_nhwc_mask; (N, HW, C/32) uint32,
+ *      required) in place of `out`.
+ *   gg_styled_tail_backward_mask_nhwc: g_raw of gg_styled_tail_backward_nhwc (same operations, same order) with act'(out)
+ *      read from the sign mask: one pass over (g_xs, mask) -> g_raw, no sums, no workspace.  C % 32 == 0.
  * ---------------------------------------------------------------------------------------------- */
 GG_API int gg_styled_tail_nhwc(void* out, void* xs, float* rgb, const void* raw, const float* noise,
                                const float* noise_weight, const float* bias, const float* demod, const float* s_next,
@@ -339,6 +351,14 @@ GG_API int gg_styled_tail_backward_nhwc(void* g_raw, float* d_s_next, float* d_d
                                         const float* s_next, const float* demod, const float* wm, int dtype,
                                         float alpha, float scale, int64_t N, int C, int64_t HW, int64_t reduce_pitch,
                                         void* stream);
+GG_API int gg_styled_tail_mask_nhwc(void* mask, void* xs, float* rgb, const void* raw, const float* noise,
+                                    const float* noise_weight, const float* bias, const float* demod,
+                                    const float* s_next, const float* wm, const float* rgb_bias, const float* skip,
+                                    int dtype, int act, float alpha, float scale, int64_t N, int C, int64_t HW,
+                                    void* stream);
+GG_API int gg_styled_tail_backward_mask_nhwc(void* g_raw, const void* g_xs, const float* g_rgb, const void* mask,
+                                             const float* s_next, const float* demod, const float* wm, int dtype,
+                                             float alpha, float scale, int64_t N, int C, int64_t HW, void* stream);
 
 /* to-RGB on channels-last activations (reference models/stylegan2/networks.py:389-405 `ToRGB.forward`: a 1x1 modulated
  * convolution without demodulation + bias + the up-sampled skip image; the reference builds B filter banks and runs a

@@ -414,7 +414,35 @@ int gg_styled_tail_backward_nhwc(void* g_raw, float* d_s_next, float* d_demod, f
                                  float scale, int64_t N, int C, int64_t HW, int64_t reduce_pitch, void* stream) {
   if (N < 0 || C < 0 || HW < 0) return fail(GG_ERR_BAD_ARG, "styled_tail_backward_nhwc: negative size");
   if (dtype != GG_F32 && dtype != GG_BF16) return fail(GG_ERR_UNSUPPORTED, "styled_tail_backward_nhwc: dtype %d not supported", dtype);
-  if (N * HW * C == 0) return GG_OK;
+  // rows of the reduction block: d_s_next, d_demod, d_wm[3] (each present only when requested)
+  int r = 0;
+  const int r_ds = d_s_next ? r++ : -1;
+  const int r_dd = d_demod ? r++ : -1;
+  const int r_gw = d_wm ? r : -1;
+  if (d_wm) r += 3;
+  if (r > 0 && reduce_pitch != C && reduce_pitch != 0 && reduce_pitch != r * C)
+    return fail(GG_ERR_BAD_ARG, "styled_tail_backward_nhwc: reduce_pitch must be C (separate dense outputs) or r*C (packed block)");
+  // the caller's destinations are slices of one (N, r, C) block when they are laid out that way (the Python face allocates
+  // them so); otherwise each is a dense (N, rows, C) tensor of its own
+  float* first = d_s_next ? d_s_next : (d_demod ? d_demod : d_wm);
+  const bool packed = r > 0 && (!d_s_next || d_s_next == first + static_cast<int64_t>(r_ds) * C) &&
+                      (!d_demod || d_demod == first + static_cast<int64_t>(r_dd) * C) &&
+                      (!d_wm || d_wm == first + static_cast<int64_t>(r_gw) * C) && reduce_pitch == r * C;
+  auto st = static_cast<cudaStream_t>(stream);
+  if (N * HW * C == 0) {
+    if (r > 0 && N * C > 0) {   // a sum over no pixels is 0
+      cudaError_t e = cudaSuccess;
+      if (packed) {
+        e = cudaMemsetAsync(first, 0, N * r * C * sizeof(float), st);
+      } else {
+        if (d_s_next && e == cudaSuccess) e = cudaMemsetAsync(d_s_next, 0, N * C * sizeof(float), st);
+        if (d_demod && e == cudaSuccess) e = cudaMemsetAsync(d_demod, 0, N * C * sizeof(float), st);
+        if (d_wm && e == cudaSuccess) e = cudaMemsetAsync(d_wm, 0, N * 3 * C * sizeof(float), st);
+      }
+      if (e != cudaSuccess) return cuda_fail(e, "styled_tail_backward_nhwc memset");
+    }
+    return GG_OK;
+  }
   const int V = dtype == GG_BF16 ? 8 : 4;
   if (C % V != 0 || C / V > kT) return fail(GG_ERR_UNSUPPORTED, "styled_tail_backward_nhwc: C must be a multiple of %d, <= %d", V, V * kT);
   if (!g_raw || !out_saved || (!g_xs && !g_rgb)) return fail(GG_ERR_BAD_ARG, "styled_tail_backward_nhwc: null tensor");
@@ -434,15 +462,9 @@ int gg_styled_tail_backward_nhwc(void* g_raw, float* d_s_next, float* d_demod, f
   p.g_raw = g_raw; p.partial = static_cast<float*>(workspace); p.g_xs = g_xs; p.out = out_saved;
   p.raw = d_demod ? raw : nullptr; p.s_next = s_next; p.demod = demod; p.g_rgb = g_rgb; p.wm = wm;
   p.alpha = alpha; p.gain = scale; p.C = C; p.hw = HW; p.chunk = static_cast<int>(chunk64); p.chunks_per_sample = K;
-  int r = 0;
-  p.r_ds = d_s_next ? r++ : -1;
-  p.r_dd = d_demod ? r++ : -1;
-  p.r_gw = d_wm ? r : -1;
-  if (d_wm) r += 3;
-  p.n_red = r;
+  p.r_ds = r_ds; p.r_dd = r_dd; p.r_gw = r_gw; p.n_red = r;
   const int lanes_p = kT / cv > 0 ? kT / cv : 1;
   const size_t smem = static_cast<size_t>(lanes_p) * (r > 0 ? r : 1) * C * sizeof(float);
-  auto st = static_cast<cudaStream_t>(stream);
   if (smem > 48 * 1024) {
     static DeviceOnce configured;
     if (configured.needed()) {
@@ -458,12 +480,7 @@ int gg_styled_tail_backward_nhwc(void* g_raw, float* d_s_next, float* d_demod, f
   else styled_tail_bwd_nhwc_kernel<__nv_bfloat16, false><<<static_cast<unsigned>(grid), kT, smem, st>>>(p);
   GG_CHECK_LAUNCH("styled_tail_backward_nhwc launch");
   if (r > 0) {
-    // partial is [N][K][r*C]: ONE finish launch writes every requested sum.  The caller's destinations are slices of one
-    // (N, r, C) block when they are laid out that way (the Python face allocates them so); otherwise one launch per sum.
-    float* first = d_s_next ? d_s_next : (d_demod ? d_demod : d_wm);
-    const bool packed = (!d_s_next || d_s_next == first + static_cast<int64_t>(p.r_ds) * C) &&
-                        (!d_demod || d_demod == first + static_cast<int64_t>(p.r_dd) * C) &&
-                        (!d_wm || d_wm == first + static_cast<int64_t>(p.r_gw) * C) && reduce_pitch == r * C;
+    // partial is [N][K][r*C]: ONE finish launch writes every requested sum of a packed block; otherwise one launch per sum
     if (packed) {
       nhwc_finish_kernel<<<static_cast<unsigned>(N * ((r * C + 31) / 32)), dim3(32, 32), 0, st>>>(
           first, static_cast<const float*>(workspace), N, K, r * C, r * C);
@@ -472,8 +489,6 @@ int gg_styled_tail_backward_nhwc(void* g_raw, float* d_s_next, float* d_demod, f
         nhwc_finish_kernel<<<static_cast<unsigned>(N * ((rows_n * C + 31) / 32)), dim3(32, 32), 0, st>>>(
             dst, static_cast<const float*>(workspace) + static_cast<int64_t>(row) * C, N, K, rows_n * C, r * C);
       };
-      if (reduce_pitch != C && reduce_pitch != 0 && reduce_pitch != r * C)
-        return fail(GG_ERR_BAD_ARG, "styled_tail_backward_nhwc: reduce_pitch must be C (separate dense outputs) or r*C (packed block)");
       if (d_s_next) finish_row(d_s_next, p.r_ds, 1);
       if (d_demod) finish_row(d_demod, p.r_dd, 1);
       if (d_wm) finish_row(d_wm, p.r_gw, 3);

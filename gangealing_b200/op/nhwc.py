@@ -164,10 +164,25 @@ def channel_scale(x, s, y=None):
     return out, dot
 
 
+def _activation_like(t, like, who, name):
+    """The styled tails read `t` 16 bytes at a time as a channels-last (N, C, H, W) tensor of `like`'s shape and dtype."""
+    if t is not None and (t.shape != like.shape or t.dtype != like.dtype or not t.is_contiguous(memory_format=CL)
+                          or not _lib.aligned16(t)):
+        raise RuntimeError("%s: %s must be a 16-byte-aligned channels-last tensor of the activation's shape and dtype"
+                           % (who, name))
+
+
+def _rgb_grad_ok(g_rgb, n, h, w, who):
+    """The styled tails' backward reads the to-RGB gradient as planar (N, 3, H*W) fp32."""
+    if g_rgb is not None and (g_rgb.shape != (n, 3, h, w) or g_rgb.dtype != torch.float32 or not g_rgb.is_contiguous()):
+        raise RuntimeError("%s: g_rgb must be a dense fp32 (N, 3, H, W) tensor" % who)
+
+
 def styled_tail(raw, noise, noise_weight, bias, demod, s_next, wm, rgb_bias, skip, want_out, negative_slope, gain, act=3,
                 want_mask=False):
     """gg_styled_tail_nhwc -> (out or None, xs or None, rgb or None).  want_mask: gg_styled_tail_mask_nhwc, the first
     result is the sign mask of the activation instead of the activation."""
+    _activation_like(raw, raw, "styled_tail", "raw")
     n, c, h, w = raw.shape
     if want_mask:
         out = sign_mask_empty(n, c, h, w, raw.device)
@@ -197,10 +212,13 @@ def styled_tail_backward(g_xs, g_rgb, out_saved, raw, s_next, demod, wm, want_ds
     n, c, h, w = out_saved.shape
     lib = _lib.load()
     dev = out_saved.device
-    g_raw = torch.empty_like(out_saved)
     want_ds = want_ds and g_xs is not None
     want_dd = want_dd and raw is not None
     want_dwm = want_dwm and g_rgb is not None
+    for name, t in (("out_saved", out_saved), ("g_xs", g_xs), ("raw", raw if want_dd else None)):
+        _activation_like(t, out_saved, "styled_tail_backward", name)
+    _rgb_grad_ok(g_rgb, n, h, w, "styled_tail_backward")
+    g_raw = torch.empty_like(out_saved)
     # the requested sums are row slices of ONE (N, R, C) block: a single finish launch, views handed to autograd
     rows = int(want_ds) + int(want_dd) + 3 * int(want_dwm)
     block = torch.empty((n, rows, c), dtype=torch.float32, device=dev) if rows else None
@@ -232,12 +250,8 @@ def styled_tail_backward_mask(g_xs, g_rgb, mask, s_next, demod, wm, negative_slo
     n, h, w, words = mask.shape
     c = 32 * words
     g_raw = torch.empty((n, c, h, w), dtype=dtype, device=mask.device, memory_format=CL)
-    if g_xs is not None and (g_xs.shape != g_raw.shape or g_xs.dtype != dtype or not g_xs.is_contiguous(memory_format=CL)
-                             or not _lib.aligned16(g_xs)):
-        raise RuntimeError("styled_tail_backward_mask: g_xs must be a 16-byte-aligned channels-last tensor of the "
-                               "activation's shape and dtype")
-    if g_rgb is not None and (g_rgb.shape != (n, 3, h, w) or g_rgb.dtype != torch.float32 or not g_rgb.is_contiguous()):
-        raise RuntimeError("styled_tail_backward_mask: g_rgb must be a dense fp32 (N, 3, H, W) tensor")
+    _activation_like(g_xs, g_raw, "styled_tail_backward_mask", "g_xs")
+    _rgb_grad_ok(g_rgb, n, h, w, "styled_tail_backward_mask")
     consts = [_f32(s_next, n * c), _f32(demod, n * c), _f32(wm, n * 3 * c)]
     rc = _lib.load().gg_styled_tail_backward_mask_nhwc(g_raw.data_ptr(), _lib.ptr(g_xs), _lib.ptr(g_rgb), mask.data_ptr(),
                                                        *[_lib.ptr(t) for t in consts], _lib.dtype_code(g_raw),

@@ -335,7 +335,8 @@ GG_API int gg_blur_nhwc_mask(void* mask, void* out2, const void* in, const float
  *      gg_blur_nhwc mode 2).  `workspace`: gg_styled_tail_backward_workspace() bytes.  Deterministic reductions.
  *      reduce_pitch: floats between consecutive samples of the sum outputs -- C (each a dense (N, C) / (N, 3, C) tensor) or
  *      R*C when they are the row slices [d_s_next | d_demod | d_wm x3] (requested ones only, in that order) of ONE (N, R, C)
- *      block, which is then finished by a single launch.
+ *      block, which is then finished by a single launch.  0 is accepted for C; any other value is refused before any
+ *      device work.  HW == 0: the requested sums are 0 (a sum over no pixels).
  *   gg_styled_tail_mask_nhwc: gg_styled_tail_nhwc with the sign mask of o (see gg_blur_nhwc_mask; (N, HW, C/32) uint32,
  *      required) in place of `out`.
  *   gg_styled_tail_backward_mask_nhwc: g_raw of gg_styled_tail_backward_nhwc (same operations, same order) with act'(out)

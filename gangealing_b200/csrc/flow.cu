@@ -189,6 +189,8 @@ int gg_flow_compose_forward(float* delta_flow, float* flow, const float* low_flo
   if (N == 0) return GG_OK;
   if (!delta_flow || !low_flow || !mask) return fail(GG_ERR_BAD_ARG, "flow_compose_forward: null tensor");
   if (flow && !identity_flow) return fail(GG_ERR_BAD_ARG, "flow_compose_forward: flow output needs identity_flow");
+  if (!aligned8(delta_flow) || !aligned8(flow) || !aligned8(low_flow) || !aligned8(identity_flow))
+    return fail(GG_ERR_BAD_ARG, "flow_compose_forward: low_flow, identity_flow, delta_flow and flow must be 8-byte aligned");
   FlowParams p{N, H, W, S};
   const int64_t total = N * S * S * H * static_cast<int64_t>(W);
   flow_compose_fwd_kernel<<<grid_for(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
@@ -205,9 +207,19 @@ int gg_flow_compose_backward(float* grad_mask, float* grad_low_flow, float* grad
   if (N == 0) return GG_OK;
   if (!low_flow || !mask) return fail(GG_ERR_BAD_ARG, "flow_compose_backward: null tensor");
   if (grad_flow && base_warp && !identity_flow) return fail(GG_ERR_BAD_ARG, "flow_compose_backward: identity_flow required");
+  const bool base_terms = grad_base_warp && grad_flow && base_warp;
+  if (base_terms && N > 0x7fffffffLL) return fail(GG_ERR_BAD_ARG, "flow_compose_backward: too many samples");
+  if (!aligned8(grad_low_flow) || !aligned8(grad_delta) || !aligned8(grad_flow) || !aligned8(low_flow) ||
+      !aligned8(identity_flow))
+    return fail(GG_ERR_BAD_ARG,
+                "flow_compose_backward: grad_low_flow, grad_delta, grad_flow, low_flow and identity_flow must be 8-byte aligned");
   FlowParams p{N, H, W, S};
   const int64_t total = N * S * S * H * static_cast<int64_t>(W);
   auto st = static_cast<cudaStream_t>(stream);
+  if (grad_base_warp && !base_terms) {   // no gradient reaches the composed grid through a base warp: d base = 0
+    const cudaError_t e = cudaMemsetAsync(grad_base_warp, 0, static_cast<size_t>(N) * 6 * sizeof(float), st);
+    if (e != cudaSuccess) return cuda_fail(e, "flow_compose_backward: zeroing grad_base_warp");
+  }
   if (grad_mask)
     flow_compose_bwd_kernel<<<grid_for(total, 256), 256, 0, st>>>(grad_mask, grad_delta, grad_flow, low_flow, mask, identity_flow,
                                                              base_warp, alpha, p, total);
@@ -216,8 +228,7 @@ int gg_flow_compose_backward(float* grad_mask, float* grad_low_flow, float* grad
     flow_low_bwd_kernel<<<grid_for(entries * 32, 256), 256, 0, st>>>(grad_low_flow, grad_delta, grad_flow, low_flow, mask,
                                                                  identity_flow, base_warp, alpha, p, entries);
   }
-  if (grad_base_warp && grad_flow && base_warp) {
-    if (N > 0x7fffffffLL) return fail(GG_ERR_BAD_ARG, "flow_compose_backward: too many samples");
+  if (base_terms) {
     flow_base_bwd_kernel<<<static_cast<unsigned>(N), kBaseThreads, 0, st>>>(grad_base_warp, grad_delta, grad_flow, low_flow,
                                                                            mask, identity_flow, base_warp, alpha, p);
   }

@@ -792,6 +792,7 @@ int lerp_args(const char* who, const float* base, int64_t base_stride, const flo
   if (base_stride != 0 && base_stride != static_cast<int64_t>(ho) * wo * 2)
     return fail(GG_ERR_BAD_ARG, "%s: base_stride must be 0 (one broadcast base grid) or ho*wo*2", who);
   if (!base || !target || !alphas) return fail(GG_ERR_BAD_ARG, "%s: null grid or alphas", who);
+  if (!aligned8(base) || !aligned8(target)) return fail(GG_ERR_BAD_ARG, "%s: base and target must be 8-byte aligned", who);
   return GG_OK;
 }
 
@@ -891,6 +892,7 @@ int gg_warp_sample_indices(int32_t* indices, const float* grid, int64_t N, int h
   const int64_t total = N * ho * static_cast<int64_t>(wo);
   if (total == 0) return GG_OK;
   if (!indices || !grid) return fail(GG_ERR_BAD_ARG, "warp_sample_indices: null tensor");
+  if (!aligned8(grid)) return fail(GG_ERR_BAD_ARG, "warp_sample_indices: grid must be 8-byte aligned");
   if (reinterpret_cast<uintptr_t>(indices) & 15) return fail(GG_ERR_BAD_ARG, "warp_sample_indices: indices must be 16-byte aligned");
   sample_indices_kernel<<<grid_for(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<int4*>(indices), grid, wp, total);
@@ -907,6 +909,7 @@ int gg_mipmap_warp_forward(void* out, float* levels_out, const void* src, const 
   const int64_t total = N * ho * static_cast<int64_t>(wo);
   if (total == 0 || C == 0) return GG_OK;
   if (!out || !src || !grid || (extra_levels > 0 && !pyramid)) return fail(GG_ERR_BAD_ARG, "mipmap_warp_forward: null tensor");
+  if (!aligned8(grid)) return fail(GG_ERR_BAD_ARG, "mipmap_warp_forward: grid must be 8-byte aligned");
   ComposeParams cp{};
   cp.grid = grid;
   return sample_forward(out, levels_out, src, pyramid, cp, wp, 0, dtype, "mipmap_warp_forward", static_cast<cudaStream_t>(stream));
@@ -929,7 +932,10 @@ int gg_stn_sample_forward(void* out, float* grid_out, float* delta_out, float* l
     if (!low || !mask || !identity) return fail(GG_ERR_BAD_ARG, "stn_sample: flow mode needs low, mask and identity");
     if (s < 1 || lh < 1 || lw < 1 || lh * s != ho || lw * s != wo)
       return fail(GG_ERR_BAD_ARG, "stn_sample: the flow grid (%d x %d, x%d) must match the output size (%d x %d)", lh, lw, s, ho, wo);
+    if (!aligned8(low) || !aligned8(identity) || !aligned8(delta_out))
+      return fail(GG_ERR_BAD_ARG, "stn_sample: low, identity and delta_out must be 8-byte aligned");
   }
+  if (!aligned8(grid_out)) return fail(GG_ERR_BAD_ARG, "stn_sample: grid_out must be 8-byte aligned");
   ComposeParams cp{};
   cp.theta = theta; cp.low = low; cp.mask = mask; cp.identity = identity; cp.alpha = alpha;
   cp.lh = lh; cp.lw = lw; cp.s = s; cp.grid_out = grid_out; cp.delta_out = delta_out;
@@ -948,6 +954,7 @@ int gg_mipmap_warp_lerp_forward(void* out, float* grid_out, const void* src, con
   const int64_t total = N * ho * static_cast<int64_t>(wo);
   if (total == 0 || C == 0) return GG_OK;
   if (!out || !src || (extra_levels > 0 && !pyramid)) return fail(GG_ERR_BAD_ARG, "mipmap_warp_lerp_forward: null tensor");
+  if (!aligned8(grid_out)) return fail(GG_ERR_BAD_ARG, "mipmap_warp_lerp_forward: grid_out must be 8-byte aligned");
   ComposeParams cp{};
   cp.base = base; cp.base_stride = base_stride; cp.target = target; cp.alpha = alphas; cp.frames = T; cp.grid_out = grid_out;
   return sample_forward(out, nullptr, src, pyramid, cp, wp, 3, dtype, "mipmap_warp_lerp_forward",
@@ -1000,6 +1007,7 @@ int gg_mipmap_warp_backward(float* grad_src, float* grad_pyramid, float* grad_gr
   if (!grad_out || !src || !grid || (extra_levels > 0 && !pyramid)) return fail(GG_ERR_BAD_ARG, "mipmap_warp_backward: null tensor");
   if (grad_src && extra_levels > 0 && !grad_pyramid) return fail(GG_ERR_BAD_ARG, "mipmap_warp_backward: grad_src needs grad_pyramid");
   if (!grad_src && !grad_grid) return GG_OK;
+  if (!aligned8(grid) || !aligned8(grad_grid)) return fail(GG_ERR_BAD_ARG, "mipmap_warp_backward: grid and grad_grid must be 8-byte aligned");
   auto st = static_cast<cudaStream_t>(stream);
   const int gridsz = grid_for(total, 256);
 #define GG_BWD(T_)                                                                                               \

@@ -13,11 +13,9 @@ from .. import _lib
 
 
 def _f32c(t):
-    if t is None:
-        return None
-    if t.dtype != torch.float32 or not t.is_contiguous():
-        t = t.float().contiguous()
-    return t
+    """`t` as a contiguous fp32 tensor with 16-byte-aligned data (None stays None).  The kernels read flows and grids as
+    float2; a contiguous view such as `buf[1:].view(n, h, w, 2)` starts 4 bytes off and is copied."""
+    return None if t is None else _lib.dense_f32(t)
 
 
 def flow_meta(low, mask, base):
@@ -56,7 +54,7 @@ def flow_grads(flow_in, like, s, g_delta, g_flow, need_low, need_mask, need_base
     n, h, w, _ = low.shape
     g_mask = torch.empty_like(mask) if need_mask else None
     g_low = torch.zeros_like(low) if need_low else None
-    g_base = torch.zeros((n, 2, 3), dtype=torch.float32, device=low.device) if (need_base and base is not None) else None
+    g_base = torch.empty((n, 2, 3), dtype=torch.float32, device=low.device) if (need_base and base is not None) else None
     rc = _lib.load().gg_flow_compose_backward(_lib.ptr(g_mask), _lib.ptr(g_low), _lib.ptr(g_base), _lib.ptr(g_delta),
                                               _lib.ptr(g_flow), low.data_ptr(), mask.data_ptr(), _lib.ptr(ident),
                                               _lib.ptr(base), _lib.ptr(alpha), n, h, w, s, _lib.stream())

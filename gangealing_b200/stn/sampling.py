@@ -132,7 +132,7 @@ class _StnSample(Function):
                 _lib.check(lib.gg_mipmap_build_backward(grad_src.data_ptr(), grad_pyr.data_ptr(), n * c, hs, ws, extra, st),
                            "gg_mipmap_build_backward")
         if need_grid and g_grid is not None:     # the caller also used the returned grid
-            gg = g_grid.float().contiguous() if gg is None else gg + g_grid.float()
+            gg = _f32c(g_grid) if gg is None else gg + g_grid.float()
         g_grid_in = g_theta = g_low = g_mask = None
         if mode == 0:
             if need_grid_in and gg is not None:
@@ -145,7 +145,7 @@ class _StnSample(Function):
                 g_theta = torch.stack([torch.einsum("nyxi,x->ni", gg, bx), torch.einsum("nyxi,y->ni", gg, by), gg.sum(dim=(1, 2))], dim=2)
                 g_theta = g_theta.reshape(theta_info[1]).to(theta_info[0])
         else:
-            gd = g_delta.float().contiguous() if g_delta is not None else None
+            gd = _f32c(g_delta)
             if (need_low or need_mask or need_theta) and (gg is not None or gd is not None):
                 g_low, g_mask, g_theta = flow_grads(flow_in, flow_like, s, gd, gg, need_low, need_mask, need_theta)
         if grad_src is not None and grad_src.dtype != x.dtype:
@@ -180,7 +180,7 @@ def sample_indices(grid, source_hw, max_num_levels=8, min_level=0.0, padding_mod
     _lib.require_cuda(grid)
     hs, ws = int(source_hw[0]), int(source_hw[1])
     max_level, min_level, _ = clamp_levels(hs, ws, max_num_levels, min_level)
-    g = grid.detach().float().contiguous()
+    g = _f32c(grid.detach())
     n, ho, wo, _ = g.shape
     out = torch.empty(n, ho, wo, 4, dtype=torch.int32, device=g.device)
     with torch.cuda.device(g.device):
@@ -219,9 +219,9 @@ def _lerp_operands(who, inputs, base, target, alphas):
         raise RuntimeError("%s: base must be (N or 1, %d, %d, 2), got %s" % (who, ho, wo, tuple(base.shape)))
     if alphas.dim() != 1 or alphas.numel() < 1:
         raise RuntimeError("%s: alphas must be a non-empty (T,) tensor" % who)
-    b = base.float().contiguous()
+    b = _f32c(base)
     stride = 0 if (b.shape[0] == 1 and n != 1) else ho * wo * 2
-    return (inputs.contiguous(), b, stride, target.float().contiguous(), alphas.float().contiguous(), ho, wo)
+    return (inputs.contiguous(), b, stride, _f32c(target), alphas.float().contiguous(), ho, wo)
 
 
 def _pyramid(x, extra):

@@ -203,9 +203,12 @@ GG_API int gg_mipmap_warp_lerp_mean(float* acc, const void* src, const float* py
  *   low_flow (N, H, W, 2); mask (N, 9*S*S, H, W); identity_flow (S*H, S*W, 2) = F.affine_grid(identity);
  *   base_warp (N, 2, 3) or NULL; alpha (N) or NULL.  All fp32.
  *   forward : delta_flow (N, S*H, S*W, 2) and, if `flow` != NULL, flow = lerp(identity, affine(identity + delta), alpha)
- *   backward: grad_mask and grad_low_flow (written), grad_base_warp (ZERO-INITIALISED by the caller: written only when
- *             grad_flow and base_warp are given); reduced in a fixed order, without atomics, so the result is the same in
- *             every run; grad_delta / grad_flow are the incoming gradients (either may be NULL).
+ *   backward: grad_mask, grad_low_flow and grad_base_warp (written; grad_base_warp is zero unless grad_flow and
+ *             base_warp are given); reduced in a fixed order, without atomics, so the result is the same in every run;
+ *             grad_delta / grad_flow are the incoming gradients (either may be NULL).
+ *   low_flow, identity_flow, delta_flow, flow, grad_low_flow, grad_delta and grad_flow are read or written as float2:
+ *   a pointer off an 8-byte boundary is refused (GG_ERR_BAD_ARG) before any device work.  So are the float2 grids of
+ *   the samplers below (grid, grid_out, delta_out, base, target, grad_grid, and mode 2's low and identity).
  * ---------------------------------------------------------------------------------------------- */
 GG_API int gg_flow_compose_forward(float* delta_flow, float* flow, const float* low_flow, const float* mask,
                                    const float* identity_flow, const float* base_warp, const float* alpha,

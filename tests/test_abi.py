@@ -114,3 +114,55 @@ def test_misaligned_vector_operands_are_refused():
     assert refused(dll.gg_feature_distance_backward(a, a, a, a, a, m, 2, 2, 64, 16, 1e-10, None))               # weight
     # the shape contracts are still checked first
     assert dll.gg_to_rgb_nhwc_forward(a, a, m, None, None, 1, 20, 16, None) == -2
+
+
+def test_misaligned_float2_operands_are_refused():
+    """Entries whose kernels read or write flows and sampling grids as float2 refuse a pointer off an 8-byte boundary (a
+    view such as buf[1:].view(n, h, w, 2)) with a status code, before any device work."""
+    dll = _lib.load()
+    a, m = 16, 4
+
+    def refused(rc):
+        return rc == -1 and b"aligned" in dll.gg_last_error()
+    fwd = [a, a, a, a, a, None, None]        # delta, flow, low, mask, identity, base, alpha
+    for i in (0, 1, 2, 4):
+        args = list(fwd)
+        args[i] = m
+        assert refused(dll.gg_flow_compose_forward(*args, 2, 3, 3, 2, None)), i
+    bwd = [a, a, a, a, a, a, a, a, a, a]     # g_mask, g_low, g_base, g_delta, g_flow, low, mask, identity, base, alpha
+    for i in (1, 3, 4, 5, 7):
+        args = list(bwd)
+        args[i] = m
+        assert refused(dll.gg_flow_compose_backward(*args, 2, 3, 3, 2, None)), i
+    assert refused(dll.gg_warp_sample_indices(a, m, 1, 8, 8, 4, 4, 0.0, 0.0, 1, None))
+    assert refused(dll.gg_mipmap_warp_forward(a, None, a, None, m, 0, 1, 1, 8, 8, 4, 4, 0, 0.0, 0.0, 1, None))
+    flow_mode = [a, a, a, None, a, None, None, a, a, a, None]    # out, grid_out, delta_out, levels, src, pyr, theta, low, mask, identity, alpha
+    for i in (1, 2, 7, 9):
+        args = list(flow_mode)
+        args[i] = m
+        assert refused(dll.gg_stn_sample_forward(*args, 2, 0, 1, 1, 8, 8, 8, 8, 4, 4, 2, 0, 0.0, 0.0, 1, None)), i
+    assert refused(dll.gg_stn_sample_forward(a, m, None, None, a, None, a, None, None, None, None, 1, 0, 1, 1, 8, 8, 8, 8,
+                                             0, 0, 1, 0, 0.0, 0.0, 1, None))               # affine mode: grid_out
+    lerp = [a, a, a, None, a, 32, a, a]      # out, grid_out, src, pyr, base, base_stride, target, alphas
+    for i in (1, 4, 6):
+        args = list(lerp)
+        args[i] = m
+        assert refused(dll.gg_mipmap_warp_lerp_forward(*args, 1, 0, 1, 1, 8, 8, 4, 4, 0, 0.0, 0.0, 1, None)), i
+    for i in (3, 5):                        # acc, src, pyr, base, base_stride, target, alphas
+        args = [a, a, None, a, 32, a, a]
+        args[i] = m
+        assert refused(dll.gg_mipmap_warp_lerp_mean(*args, 1, 0, 1, 1, 8, 8, 4, 4, 0, 0.0, 0.0, 1, 0, None)), i
+    assert refused(dll.gg_mipmap_warp_backward(None, None, a, a, a, None, m, 0, 1, 1, 8, 8, 4, 4, 0, 0.0, 0.0, 1, None))
+    assert refused(dll.gg_mipmap_warp_backward(None, None, m, a, a, None, a, 0, 1, 1, 8, 8, 4, 4, 0, 0.0, 0.0, 1, None))
+
+
+def test_flow_backward_validates_before_its_first_launch():
+    """gg_flow_compose_backward checks every argument, the sample count of the g_base grid included, before it launches
+    the g_mask and g_low kernels (the pointers below are never dereferenced)."""
+    dll = _lib.load()
+    a = 16
+    rc = dll.gg_flow_compose_backward(a, a, a, a, a, a, a, a, a, a, 1 << 31, 1, 1, 1, None)
+    assert rc == -1 and b"too many samples" in dll.gg_last_error()
+    # identity is required when g_flow meets a base warp, whichever outputs are requested
+    assert dll.gg_flow_compose_backward(a, a, None, None, a, a, a, None, a, None, 2, 2, 2, 2, None) == -1
+    assert dll.gg_flow_compose_backward(a, a, a, a, a, None, a, a, a, a, 2, 2, 2, 2, None) == -1      # null low

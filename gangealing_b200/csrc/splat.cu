@@ -23,6 +23,8 @@
 // Float atomics make the summation order (hence the last bits) run-to-run dependent, exactly as in the
 // reference; the SET of touched pixels is deterministic.
 // HBM: algorithmic bytes 4*N*(P*(2+C) + (C+1)*H*W + 2*C*H*W); the scatter itself is L2-reduction-bound.
+#include <algorithm>
+
 #include "common.cuh"
 #include "lookup.cuh"
 
@@ -124,6 +126,109 @@ splat_normalize_kernel(float* __restrict__ out, const float* __restrict__ input,
   }
 }
 
+// ---------------------------------------------------------------------------------------------------- composited grids
+// The label-propagation animation (reference vis_correspondence.py:133-158): for every (frame, image) the two splats of
+// splat_points (helpers.py:178-187, colours and soft-normalised alpha), the alpha composite, then images2grid
+// (helpers.py:39-43: make_grid(normalize=True, range=(-1, 1)) and the uint8 quantisation), in one scatter launch and one
+// composite launch per chunk of frames.  Both splats weigh a footprint pixel with the same Gaussian a, so one pass
+// accumulates [sum a, sum a*r, sum a*g, sum a*b] and, with an alpha channel, [sum a*alpha, 0, 0, 0]: one or two 16-byte
+// reductions per footprint pixel.  Without an alpha channel sum a*alpha = sum a and the second group is not allocated.
+struct GridParams {
+  int64_t n, points;          // N images per frame, P points per image
+  int r;                      // image side
+  int xmaps, pad, hg, wg;     // make_grid layout
+  int colors_n, alpha_n;      // 1 (broadcast) or N
+  float sigma, opacity;
+};
+
+// One thread per (frame, image, point); the footprint schedule and bounds test of splat_direct_kernel.
+template <bool ALPHA>
+__global__ void __launch_bounds__(64)
+splat_frames_kernel(float* __restrict__ acc, const float* __restrict__ coords, const float* __restrict__ colors,
+                    const float* __restrict__ alpha, GridParams p, int64_t total) {
+  constexpr int SLOTS = ALPHA ? 8 : 4;
+  const int64_t index = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (index >= total) return;
+  const int64_t image = index / p.points;            // (frame, image) within the chunk
+  const int64_t pt = index - image * p.points;
+  const int64_t n = image % p.n;
+  const float2 xy = __ldg(reinterpret_cast<const float2*>(coords + index * 2));
+  const float x = xy.x, y = xy.y;
+  const int h = p.r, w = p.r;
+  if (!(x >= 0.f && x < static_cast<float>(w) && y >= 0.f && y < static_cast<float>(h))) return;
+  const float sd = p.sigma, len = 2.f * sd, norm = -1.f / (2.f * sd * sd);
+  const int t = static_cast<int>(fmaxf(0.f, floorf(y - len))), b = static_cast<int>(fminf(static_cast<float>(h - 1), ceilf(y + len)));
+  const int l = static_cast<int>(fmaxf(0.f, floorf(x - len))), r = static_cast<int>(fminf(static_cast<float>(w - 1), ceilf(x + len)));
+  const float* col = colors + ((p.colors_n == 1 ? 0 : n) * p.points + pt) * 3;
+  const float cr = __ldg(col), cg = __ldg(col + 1), cb = __ldg(col + 2);
+  const float al = ALPHA ? __ldg(alpha + (p.alpha_n == 1 ? 0 : n) * p.points + pt) : 0.f;
+  float* acc_n = acc + image * h * static_cast<int64_t>(w) * SLOTS;
+  for (int py = t; py <= b; ++py) {
+    const float ddy = static_cast<float>(py) - y;
+    float* row = acc_n + static_cast<int64_t>(py) * w * SLOTS;
+    for (int px = l; px <= r; ++px) {
+      const float ddx = static_cast<float>(px) - x;
+      const float a = expf(norm * (ddx * ddx + ddy * ddy));
+      float* dst = row + px * SLOTS;
+      red_add_v4(dst, a * 1.f, a * cr, a * cg, a * cb);
+      if (ALPHA) red_add_v4(dst + 4, a * al, 0.f, 0.f, 0.f);
+    }
+  }
+}
+
+// make_grid's normalize (clamp(-1, 1), sub(-1), div(2)) and images2grid's mul(255), add(0.5), clamp(0, 255) and
+// truncating uint8 cast, each rounded on its own.
+__device__ __forceinline__ unsigned char quantise(float v) {
+  v = fminf(fmaxf(v, -1.f), 1.f);
+  v = __fdiv_rn(__fsub_rn(v, -1.f), 2.f);
+  v = __fadd_rn(__fmul_rn(v, 255.f), 0.5f);
+  v = fminf(fmaxf(v, 0.f), 255.f);
+  return static_cast<unsigned char>(static_cast<int>(v));
+}
+
+// One output pixel (3 bytes, HWC) of one frame's grid per thread.  SPLAT: composite the accumulated splats over the image
+// as splat2d's normalisation and splat_points' blend do, every operation rounded on its own:
+//   obj = S_c / (A + 1e-8);  m = (S_alpha / (max(A, 1) + 1e-8)) * opacity;  v = m * obj + (1 - m) * img.
+template <bool SPLAT, bool ALPHA>
+__global__ void __launch_bounds__(256)
+composite_grid_kernel(unsigned char* __restrict__ out, const float* __restrict__ acc, const float* __restrict__ images,
+                      GridParams p, int64_t total) {
+  constexpr int SLOTS = ALPHA ? 8 : 4;
+  const int64_t idx = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (idx >= total) return;
+  const int gx = static_cast<int>(idx % p.wg);
+  const int64_t rest = idx / p.wg;
+  const int gy = static_cast<int>(rest % p.hg);
+  const int64_t frame = rest / p.hg;
+  unsigned char* o = out + idx * 3;
+  const int cell = p.r + p.pad;
+  const int yy = gy - p.pad, xx = gx - p.pad;
+  const int y = yy >= 0 ? yy % cell : -1, x = xx >= 0 ? xx % cell : -1;
+  const int64_t k = yy >= 0 && xx >= 0 ? static_cast<int64_t>(yy / cell) * p.xmaps + xx / cell : -1;
+  if (y < 0 || y >= p.r || x < 0 || x >= p.r || k < 0 || k >= p.n) {   // make_grid's padding (pad value 0)
+    o[0] = o[1] = o[2] = 0;
+    return;
+  }
+  const int64_t image = frame * p.n + k;
+  const int64_t plane = static_cast<int64_t>(p.r) * p.r, pix = static_cast<int64_t>(y) * p.r + x;
+  const float* img = images + image * 3 * plane + pix;
+  float v[3] = {__ldg(img), __ldg(img + plane), __ldg(img + 2 * plane)};
+  if (SPLAT) {
+    const float* a = acc + (image * plane + pix) * SLOTS;
+    const float4 s = __ldg(reinterpret_cast<const float4*>(a));
+    const float sa = ALPHA ? __ldg(a + 4) : s.x;
+    const float den = __fadd_rn(s.x, 1e-8f);
+    const float m = __fmul_rn(__fdiv_rn(sa, __fadd_rn(fmaxf(s.x, 1.f), 1e-8f)), p.opacity);
+    const float keep = __fsub_rn(1.f, m);
+    const float sc[3] = {s.y, s.z, s.w};
+#pragma unroll
+    for (int c = 0; c < 3; ++c) v[c] = __fadd_rn(__fmul_rn(m, __fdiv_rn(sc[c], den)), __fmul_rn(keep, v[c]));
+  }
+  o[0] = quantise(v[0]);
+  o[1] = quantise(v[1]);
+  o[2] = quantise(v[2]);
+}
+
 inline int splat_grid(int64_t total, int threads) {
   int64_t g = (total + threads - 1) / threads;
   const int64_t cap = static_cast<int64_t>(sm_count()) * 8;
@@ -194,6 +299,83 @@ int gg_splat2d_lookup_forward(float* out, float* points_out, void* workspace, co
   LookupParams lk;
   lk.grid = grid; lk.gh = grid_h; lk.gw = grid_w; lk.k = unnorm_k; lk.m = unnorm_m; lk.points_out = points_out;
   return splat_impl(out, workspace, input, query, values, sigma, N, P, C, H, W, soft_normalize, &lk, stream);
+}
+
+int64_t gg_splat_composite_grid_workspace(int64_t T_chunk, int64_t N, int R, int has_alpha) {
+  if (T_chunk < 0 || N < 0 || R < 0) return -1;
+  return T_chunk * N * R * static_cast<int64_t>(R) * (has_alpha ? 8 : 4) * static_cast<int64_t>(sizeof(float));
+}
+
+int gg_splat_composite_grid(unsigned char* out, void* workspace, int64_t workspace_bytes, const float* images,
+                            const float* points, const float* colors, const float* alpha, float sigma, float opacity,
+                            int64_t T, int64_t N, int64_t P, int C, int R, int nrow, int padding, int colors_n, int alpha_n,
+                            void* stream) {
+  constexpr int64_t kIntMax = 0x7fffffffLL;
+  if (T < 0 || N < 1 || P < 0 || R < 1 || nrow < 1 || padding < 0)
+    return fail(GG_ERR_BAD_ARG, "splat_composite_grid: T, P, padding >= 0 and N, R, nrow >= 1");
+  if (C != 3) return fail(GG_ERR_BAD_ARG, "splat_composite_grid: C must be 3 (RGB images and colours)");
+  if (!(sigma > 0.f)) return fail(GG_ERR_BAD_ARG, "splat_composite_grid: sigma must be > 0");
+  if (!(opacity >= 0.f && opacity <= 1.f)) return fail(GG_ERR_BAD_ARG, "splat_composite_grid: opacity must lie in [0, 1]");
+  if (T > 0 && (!out || !images)) return fail(GG_ERR_BAD_ARG, "splat_composite_grid: null output or images");
+  const bool splat = P > 0 && T > 0;
+  const bool has_alpha = alpha != nullptr;
+  if (splat && (!points || !colors || !workspace)) return fail(GG_ERR_BAD_ARG, "splat_composite_grid: null points, colors or workspace");
+  if (splat && (colors_n != 1 && colors_n != N)) return fail(GG_ERR_BAD_ARG, "splat_composite_grid: colors_n must be 1 or N");
+  if (splat && has_alpha && (alpha_n != 1 && alpha_n != N)) return fail(GG_ERR_BAD_ARG, "splat_composite_grid: alpha_n must be 1 or N");
+  if (splat && (reinterpret_cast<uintptr_t>(workspace) % 16 != 0))
+    return fail(GG_ERR_BAD_ARG, "splat_composite_grid: workspace must be 16-byte aligned (vector reductions)");
+  if (splat && (reinterpret_cast<uintptr_t>(points) % 8 != 0))
+    return fail(GG_ERR_BAD_ARG, "splat_composite_grid: points must be 8-byte aligned");
+  GridParams p;
+  p.n = N; p.points = P; p.r = R;
+  p.xmaps = static_cast<int>(N < nrow ? N : nrow);
+  const int64_t ymaps = (N + p.xmaps - 1) / p.xmaps;
+  p.pad = N == 1 ? 0 : padding;                      // make_grid returns a single image as it is
+  const int64_t hg = ymaps * (R + p.pad) + p.pad, wg = static_cast<int64_t>(p.xmaps) * (R + p.pad) + p.pad;
+  const int slots = has_alpha ? 8 : 4;
+  const int64_t frame_acc = N * R * static_cast<int64_t>(R) * slots;
+  if (hg * wg * 3 > kIntMax || frame_acc > kIntMax || N * 3 * R * static_cast<int64_t>(R) > kIntMax || N * P > kIntMax)
+    return fail(GG_ERR_BAD_ARG, "splat_composite_grid: one frame's grid, images, accumulators or points exceed 2^31 elements");
+  p.hg = static_cast<int>(hg); p.wg = static_cast<int>(wg);
+  p.colors_n = colors_n; p.alpha_n = alpha_n; p.sigma = sigma; p.opacity = opacity;
+  const int64_t frame_bytes = frame_acc * static_cast<int64_t>(sizeof(float));
+  // frames per launch: as many as the workspace holds, with every launch's thread count below 2^31
+  int64_t chunk = std::min(T, kIntMax / std::max(splat ? N * P : 1, hg * wg));
+  if (splat) {
+    if (workspace_bytes < frame_bytes)
+      return fail(GG_ERR_BAD_ARG, "splat_composite_grid: the workspace holds less than one frame's accumulators");
+    chunk = std::min(chunk, workspace_bytes / frame_bytes);
+  }
+  if (T == 0) return GG_OK;
+  auto st = static_cast<cudaStream_t>(stream);
+  float* acc = static_cast<float*>(workspace);
+  for (int64_t t0 = 0; t0 < T; t0 += chunk) {
+    const int64_t tc = T - t0 < chunk ? T - t0 : chunk;
+    const int64_t pix = tc * hg * wg;
+    const float* img = images + t0 * N * 3 * R * static_cast<int64_t>(R);
+    unsigned char* o = out + t0 * hg * wg * 3;
+    const unsigned blocks = static_cast<unsigned>((pix + 255) / 256);
+    if (splat) {
+      cudaError_t e = cudaMemsetAsync(acc, 0, static_cast<size_t>(tc * frame_bytes), st);
+      if (e != cudaSuccess) return cuda_fail(e, "splat_composite_grid workspace memset");
+      const int64_t total = tc * N * P;
+      const unsigned sblocks = static_cast<unsigned>((total + 63) / 64);
+      const float* pts = points + t0 * N * P * 2;
+      if (has_alpha) {
+        splat_frames_kernel<true><<<sblocks, 64, 0, st>>>(acc, pts, colors, alpha, p, total);
+        GG_CHECK_LAUNCH("splat_frames launch");
+        composite_grid_kernel<true, true><<<blocks, 256, 0, st>>>(o, acc, img, p, pix);
+      } else {
+        splat_frames_kernel<false><<<sblocks, 64, 0, st>>>(acc, pts, colors, nullptr, p, total);
+        GG_CHECK_LAUNCH("splat_frames launch");
+        composite_grid_kernel<true, false><<<blocks, 256, 0, st>>>(o, acc, img, p, pix);
+      }
+    } else {
+      composite_grid_kernel<false, false><<<blocks, 256, 0, st>>>(o, nullptr, img, p, pix);
+    }
+    GG_CHECK_LAUNCH("composite_grid launch");
+  }
+  return GG_OK;
 }
 
 }  // extern "C"

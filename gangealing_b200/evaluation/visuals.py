@@ -157,6 +157,13 @@ def smooth_congealing(t, data, label_points=None, resolution=256, length=240, fl
     image, then backward from the label itself, and the two runs are blended as the reference does (:279-287).
     -> (frames (F, N, C, R, R); points (stages * length, N, P, 2) fp32 pixel positions in the frames, or None;
         the label's unaligned-space pixel positions (N, P, 2) that the flip stage's splat uses, or None)."""
+    return _smooth_congealing(t, data, label_points, resolution, length, flip_length, vis_in_stages, stage_flip,
+                              output_resolution, classifier, cluster, num_heads, no_flip_inference, iters, padding_mode)[:3]
+
+
+def _smooth_congealing(t, data, label_points, resolution, length, flip_length, vis_in_stages, stage_flip, output_resolution,
+                       classifier, cluster, num_heads, no_flip_inference, iters, padding_mode):
+    """smooth_congealing's results and the flip decision (N,) bool."""
     ops = t.ops
     res = output_resolution or data.size(-1)
     n = data.size(0)
@@ -182,7 +189,7 @@ def smooth_congealing(t, data, label_points=None, resolution=256, length=240, fl
         frames.append(ops.mipmap_warp_lerp(data, grids[i], grids[i + 1], alphas, WARP_LEVELS)[0])
     frames = torch.cat(frames, 0)
     if label_points is None:
-        return frames, None, None
+        return frames, None, None, flip_indices
     # sample_images_and_points (:48-54) and :240-253
     points = label_points.to(data.device).unsqueeze(0).repeat(n, 1, 1)
     points_normalized = _normalize(points, res, resolution)
@@ -205,7 +212,7 @@ def smooth_congealing(t, data, label_points=None, resolution=256, length=240, fl
         rev, congealed_centers = ops.track_points_lerp(grids[-i - 1], grids[-i - 2], alphas, normalized_unaligned,
                                                        congealed_centers, patch)
         propagated[-i - 1].lerp_(rev.float().flip(0), blend)
-    return frames, torch.cat(propagated, 0), unaligned
+    return frames, torch.cat(propagated, 0), unaligned, flip_indices
 
 
 def _normalize(points, res, out_res):
@@ -214,3 +221,133 @@ def _normalize(points, res, out_res):
 
 def _unnormalize(points, res, out_res):
     return points.div((res - 1) / res).div(2).add(0.5).mul(out_res - 1)
+
+
+# ------------------------------------------------------------------------------------------------ labelled videos
+# The label-propagation, correspondence and labelled average-image videos of vis_correspondence.py as uint8 frames
+# (F, H, W, 3), the frames its save_video receives; encoding them is left to the caller.  Colours are required: the
+# reference's default Plotly colour scales (get_plotly_colors) are not reproduced here.
+PAUSE_STEPS, INTERP_STEPS, END_PAUSE_STEPS = 60, 60, 5    # visualize_correspondence (:121-123), average_and_congeal (:428-433)
+
+
+def _ops_or_cuda(ops):
+    if ops is not None:
+        return ops
+    from ..opset import cuda_ops
+    return cuda_ops()
+
+
+def _label_inputs(colors, alpha_channel):
+    colors = colors.unsqueeze(0) if colors.dim() == 2 else colors
+    if alpha_channel is not None and alpha_channel.dim() == 2:
+        alpha_channel = alpha_channel.unsqueeze(0)
+    return colors, alpha_channel
+
+
+def _splat_points(ops, images, points, colors, alpha_channel, sigma, opacity):
+    """splat_points (helpers.py:134-194, alpha blending) on the op set's splat2d: points (N, P, 2) pixels, colors and
+    alpha_channel (N or 1, P, C)."""
+    n, _, h, w = images.shape
+    p = points.size(1)
+    if alpha_channel is None:
+        alpha_channel = torch.ones(n, p, 1, device=images.device)
+    sig = torch.full((n,), float(sigma), device=images.device)
+    obj = ops.splat2d(torch.zeros(n, 3, h, w, device=images.device), points.float().contiguous(),
+                      colors.expand(n, p, 3).float().contiguous(), sig, False)
+    mask = ops.splat2d(torch.zeros(n, 1, h, w, device=images.device), points.float().contiguous(),
+                       alpha_channel.expand(n, p, 1).float().contiguous(), sig, True) * opacity
+    return mask * obj + (1 - mask) * images
+
+
+@torch.no_grad()
+def label_propagation_frames(frames, points, colors, alpha_channel=None, sigma=1.2, opacity=0.7, initial_frames=None,
+                             ops=None):
+    """visualize_label_propagation (vis_correspondence.py:133-158): the label splatted at its tracked points onto every
+    tracked frame, each frame's images laid out by images2grid with nrow = int(sqrt(N)), `initial_frames` first, and the
+    whole video reversed.  frames (T, N, 3, R, R): smooth_congealing's frames without the flip stage's first
+    flip_length; points (T, N, P, 2): smooth_congealing's tracked points; colors (N or 1, P, 3) in [-1, 1] (required)
+    and alpha_channel (N or 1, P, 1) or None; initial_frames (F0, Hg, Wg, 3) uint8 or None.  One splat_composite_grid
+    call of the op set (cuda_ops() by default).  -> (F0 + T, Hg, Wg, 3) uint8."""
+    ops = _ops_or_cuda(ops)
+    colors, alpha_channel = _label_inputs(colors, alpha_channel)
+    nrow = int(math.sqrt(frames.size(1)))
+    out = ops.splat_composite_grid(frames, points, colors, alpha_channel, sigma, opacity, nrow)
+    if initial_frames is not None:
+        out = torch.cat([initial_frames.to(out.device), out], 0)
+    return out.flip(0)
+
+
+@torch.no_grad()
+def smooth_correspondence(t, data, label_points, colors, alpha_channel=None, sigma=1.2, opacity=0.7,
+                          **smooth_congealing_kwargs):
+    """smoothly_congeal_and_propagate's three videos (vis_correspondence.py:208-298, :118-130): the congealing
+    animation of `data`, the propagation of the dense label (label_points (P, 2) at `resolution`, as smooth_congealing)
+    and the correspondence video that joins them.  With stage_flip, the propagation starts with the label splatted at its
+    unclamped unaligned points onto the images sampled on the identity grid, flipped as the images are (:263-271).
+    The correspondence video is the congealing frames, 60 pauses on the last one, 60 frames blending it into the first
+    propagation frame (float lerp, clamp(0, 255), round, on the host as the reference does), the propagation frames and 5
+    pauses on the last one.  Every grid comes from the op set's splat_composite_grid.  colors (N or 1, P, 3) are
+    required; alpha_channel (N or 1, P, 1) or None.  smooth_congealing_kwargs: smooth_congealing's keyword arguments.
+    -> dict of uint8 (F, Hg, Wg, 3) tensors on data's device: congealing, propagation, correspondence."""
+    kw = dict(resolution=256, length=240, flip_length=40, vis_in_stages=False, stage_flip=False, output_resolution=None,
+              classifier=None, cluster=None, num_heads=1, no_flip_inference=False, iters=1, padding_mode="border")
+    unknown = set(smooth_congealing_kwargs) - set(kw)
+    if unknown:
+        raise TypeError("smooth_correspondence: unexpected keyword arguments %s" % sorted(unknown))
+    kw.update(smooth_congealing_kwargs)
+    ops = t.ops
+    colors, alpha_channel = _label_inputs(colors, alpha_channel)
+    frames, points, unaligned, flip_indices = _smooth_congealing(t, data, label_points, **kw)
+    n, res = data.size(0), frames.size(-1)
+    nrow = int(math.sqrt(n))
+    congealing = ops.splat_composite_grid(frames, None, None, None, sigma, opacity, nrow)
+    initial, tracked = None, frames
+    if kw["stage_flip"]:
+        tracked = frames[kw["flip_length"]:]
+        identity = _identity(n, res, data)
+        images = ops.mipmap_warp(data, identity, WARP_LEVELS)[0]
+        splatted = _splat_points(ops, images, unaligned, colors, alpha_channel, sigma, opacity)
+        flipped = ops.mipmap_warp_lerp(splatted, identity, flip_grid(identity, flip_indices),
+                                       cosine_alphas(kw["flip_length"], data.device), WARP_LEVELS)[0]
+        initial = ops.splat_composite_grid(flipped, None, None, None, sigma, opacity, nrow)
+    propagation = label_propagation_frames(tracked, points, colors, alpha_channel, sigma, opacity, initial, ops=ops)
+    blend = torch.linspace(0, 1, steps=INTERP_STEPS).view(INTERP_STEPS, 1, 1, 1)
+    interp = congealing[-1:].cpu().float().lerp(propagation[:1].cpu().float(), blend).clamp(0, 255).round().to(torch.uint8)
+    correspondence = torch.cat([congealing, congealing[-1:].expand(PAUSE_STEPS, -1, -1, -1), interp.to(congealing.device),
+                                propagation, propagation[-1:].expand(END_PAUSE_STEPS, -1, -1, -1)], 0)
+    return {"congealing": congealing, "propagation": propagation, "correspondence": correspondence}
+
+
+def _minmax_normalize(images, amin=None, amax=None):
+    """utils/vis_tools/helpers.py:26-36 `normalize`: per-image min/max, or clamp to the given range."""
+    if amin is None:
+        amin, amax = images.amin(dim=(1, 2, 3), keepdim=True), images.amax(dim=(1, 2, 3), keepdim=True)
+    else:
+        amin, amax = torch.tensor(amin, device=images.device), torch.tensor(amax, device=images.device)
+        images = images.clamp(amin, amax)
+    return images.sub(amin).div(torch.maximum(amax - amin, torch.tensor(1e-5, device=images.device)))
+
+
+@torch.no_grad()
+def labeled_average_frames(average_frames, label_points, colors, alpha_channel=None, sigma=1.2, opacity=0.7,
+                           resolution=256, ops=None):
+    """The average-image video of average_and_congeal with its labelled tail (vis_correspondence.py:420-437): the frames
+    min/max-normalised one by one; the label splatted onto the last frame (splat_points on the op set's splat2d); 60
+    pauses on the last frame, 60 frames blending it into the labelled frame, 5 pauses on that; then mul(255).round().
+    average_frames (F, 3, R, R): congealing_average_frames' frames; label_points (P, 2) integer pixels at `resolution`
+    (converted to R and rounded as sample_images_and_points does); colors (1, P, 3) in [-1, 1] (required) and
+    alpha_channel (1, P, 1) or None.  The op set is cuda_ops() by default.  -> (F + 125, R, R, 3) uint8."""
+    ops = _ops_or_cuda(ops)
+    colors, alpha_channel = _label_inputs(colors, alpha_channel)
+    frames = _minmax_normalize(average_frames.float())
+    res = frames.size(-1)
+    points = label_points.to(frames.device)
+    if resolution != res:
+        points = _unnormalize(_normalize(points, res, resolution), res, res).round().long()
+    last = frames[-1:].mul(2).add(-1)
+    labeled = _splat_points(ops, last, points.float().unsqueeze(0), colors, alpha_channel, sigma, opacity)
+    blend = torch.linspace(0, 1, steps=INTERP_STEPS, device=frames.device).view(INTERP_STEPS, 1, 1, 1)
+    interp = _minmax_normalize(last.lerp(labeled, blend), -1, 1)
+    frames = torch.cat([frames, frames[-1:].repeat(PAUSE_STEPS, 1, 1, 1), interp,
+                        interp[-1:].repeat(END_PAUSE_STEPS, 1, 1, 1)], 0)
+    return frames.mul(255.0).round().permute(0, 2, 3, 1).to(torch.uint8)

@@ -21,6 +21,7 @@ def cuda_ops():
         from .splat2d import splat2d as _splat2d
         from .splat2d import splat2d_lookup as _splat2d_lookup
         from .splat2d import track_points_lerp as _track_points_lerp
+        from .splat2d import splat_composite_grid as _splat_composite_grid
         from .splat2d import laplacian_blend as _laplacian_blend
         from .op import feature_distance as _fd
         from .op import vgg_pool as _vp
@@ -57,5 +58,6 @@ def cuda_ops():
             mipmap_warp_lerp=_smp.mipmap_warp_lerp,       # congealing animation: T lerped-grid warps from one pyramid
             mipmap_warp_lerp_mean=_smp.mipmap_warp_lerp_mean,   # ... and their per-frame batch sums, frames never written
             track_points_lerp=_track_points_lerp,         # dense point tracking over a stage's frames, one launch
+            splat_composite_grid=_splat_composite_grid,   # label propagation: splats + composite + uint8 grid per frame
         )
     return _cached

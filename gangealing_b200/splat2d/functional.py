@@ -8,7 +8,7 @@ import torch.autograd as ag
 
 from .. import _lib
 
-__all__ = ["splat2d", "splat2d_lookup", "nn_argmin", "track_points_lerp"]
+__all__ = ["splat2d", "splat2d_lookup", "nn_argmin", "track_points_lerp", "splat_composite_grid"]
 
 
 class Splat2DFunction(ag.Function):
@@ -123,3 +123,50 @@ def track_points_lerp(base, target, alphas, points, centers, patch_size):
                                                 pts.data_ptr(), t, n, points.size(1), h, w, int(patch_size), _lib.stream()),
                "gg_track_points_lerp")
     return track, c
+
+
+@torch.no_grad()
+def splat_composite_grid(images, points, colors, alpha_channel, sigma, opacity, nrow, max_workspace_bytes=1 << 29,
+                         padding=2):
+    """The label-propagation animation's frames (reference vis_correspondence.py:133-158): for every frame t,
+    splat_points(images[t], points[t], sigma, opacity, colors, alpha_channel) (utils/vis_tools/helpers.py:134-194, alpha
+    blending) then images2grid(nrow=nrow, normalize=True, range=(-1, 1)) (helpers.py:39-43), in one scatter and one
+    composite launch per chunk of frames (csrc/splat.cu).
+    images (T, N, 3, R, R) fp32; points (T, N, P, 2) pixel (x, y) or None (then the frames' images2grid); colors
+    (N or 1, P, 3) and alpha_channel (N or 1, P, 1) or None, broadcast over the frames.  The frames are splatted in chunks
+    whose accumulators fit max_workspace_bytes (T_chunk * N * R^2 * 16 bytes, 32 with an alpha channel).
+    -> (T, Hg, Wg, 3) uint8 on the device, make_grid's layout (a single image without padding)."""
+    _lib.require_cuda(images, points, colors, alpha_channel)
+    if images.dim() != 5 or images.size(2) != 3 or images.size(3) != images.size(4):
+        raise RuntimeError("splat_composite_grid: images must be (T, N, 3, R, R)")
+    t, n, _, r, _ = images.shape
+    p = 0
+    if points is not None:
+        if points.dim() != 4 or tuple(points.shape[:2]) != (t, n) or points.size(3) != 2:
+            raise RuntimeError("splat_composite_grid: points must be (T, N, P, 2) with (T, N) = (%d, %d)" % (t, n))
+        p = points.size(2)
+        if colors is None:
+            raise ValueError("splat_composite_grid: colors is required (plotly colour scales are not supported)")
+    counts = []
+    for name, v, c in (("colors", colors, 3), ("alpha_channel", alpha_channel, 1)):
+        if v is not None and (v.dim() != 3 or v.size(0) not in (1, n) or v.size(1) != p or v.size(2) != c):
+            raise RuntimeError("splat_composite_grid: %s must be (N or 1, P, %d) with N = %d, P = %d" % (name, c, n, p))
+        counts.append(v.size(0) if v is not None else 1)
+    images = images.float().contiguous()
+    points, colors, alpha_channel = [None if (v is None or p == 0) else v.float().contiguous()
+                                     for v in (points, colors, alpha_channel)]
+    lib = _lib.load()
+    xmaps = min(nrow, n)
+    pad = 0 if n == 1 else padding
+    hg, wg = -(-n // xmaps) * (r + pad) + pad, xmaps * (r + pad) + pad
+    out = torch.empty((t, hg, wg, 3), dtype=torch.uint8, device=images.device)
+    ws, ws_bytes = None, 0
+    if p > 0 and t > 0:
+        frame = lib.gg_splat_composite_grid_workspace(1, n, r, int(alpha_channel is not None))
+        ws_bytes = frame * max(1, min(t, max_workspace_bytes // frame))
+        ws = torch.empty(ws_bytes // 4, dtype=torch.float32, device=images.device)
+    rc = lib.gg_splat_composite_grid(out.data_ptr(), _lib.ptr(ws), ws_bytes, images.data_ptr(), _lib.ptr(points),
+                                     _lib.ptr(colors), _lib.ptr(alpha_channel), float(sigma), float(opacity), t, n, p, 3, r,
+                                     int(nrow), int(padding), counts[0], counts[1], _lib.stream())
+    _lib.check(rc, "gg_splat_composite_grid")
+    return out

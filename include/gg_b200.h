@@ -236,6 +236,29 @@ GG_API int gg_splat2d_forward(float* out, void* workspace, const float* input, c
                               int W, int soft_normalize, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * gg_splat_composite_grid -- the label-propagation animation's frames (reference applications/vis_correspondence.py:133-158):
+ *   for every frame t and image n, splat_points' two splats at points[t, n] (utils/vis_tools/helpers.py:178-187; the
+ *   footprint, weight and bounds of gg_splat2d_forward at sigma), the alpha composite over images[t, n], then images2grid
+ *   (helpers.py:39-43: torchvision make_grid(nrow, padding, normalize=True, range=(-1, 1)) and the uint8 quantisation):
+ *       A = sum a, S_c = sum a * colors[c], S_alpha = sum a * alpha (= A when alpha is NULL)
+ *       v = m * (S_c / (A + 1e-8)) + (1 - m) * img,  m = (S_alpha / (max(A, 1) + 1e-8)) * opacity
+ *       out = uint8(clamp(((clamp(v, -1, 1) - (-1)) / 2) * 255 + 0.5, 0, 255))   (every operation rounded on its own)
+ *   laid out as make_grid does: xmaps = min(nrow, N), ymaps = ceil(N / xmaps), pad value 0; N == 1: the bare image.
+ *   out (T, Hg, Wg, 3) uint8; images (T, N, 3, R, R) fp32; points (T, N, P, 2) fp32 pixels (x, y), 8-byte aligned;
+ *   colors (colors_n, P, 3) and alpha (alpha_n, P, 1) fp32 or NULL, broadcast over the frames, colors_n / alpha_n 1 or N.
+ *   P == 0: points, colors and workspace may be NULL, and out is images2grid of the frames.  C must be 3.
+ *   `workspace`: 16-byte aligned, workspace_bytes of it; frames are splatted in chunks of
+ *   workspace_bytes / gg_splat_composite_grid_workspace(1, N, R, alpha != NULL) frames (at least one must fit).
+ *   Float atomics: with more than two contributions per pixel the sums' last bits depend on their order.
+ *   Arguments are validated before any device work (GG_ERR_BAD_ARG).
+ * ---------------------------------------------------------------------------------------------- */
+GG_API int64_t gg_splat_composite_grid_workspace(int64_t T_chunk, int64_t N, int R, int has_alpha);
+GG_API int gg_splat_composite_grid(unsigned char* out, void* workspace, int64_t workspace_bytes, const float* images,
+                                   const float* points, const float* colors, const float* alpha, float sigma,
+                                   float opacity, int64_t T, int64_t N, int64_t P, int C, int R, int nrow, int padding,
+                                   int colors_n, int alpha_n, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * The STN's sampling in ONE pass (north_star: "antialiased bilinear grid_sample fused with flow-compose in one pass").
  * The sampling grid is generated per output pixel from the head's raw outputs instead of being read from memory:
  *   mode 1  SimilarityHead (reference warping_heads.py:120-136): grid = F.affine_grid(theta (N, 2, 3), align_corners=False)

@@ -9,7 +9,11 @@ Average-image animation, 512^2 source and output, two STN stages x 240 frames, b
   * congealing_average_frames end to end at n_mean images;
   * the mean kernel (gg_mipmap_warp_lerp_mean) per (sample, frame), with its DRAM bytes.
 Point tracking, N = 4, P = 40000, patch 9, 512^2 grids, 240 frames: track_points_lerp against the per-frame Unfold
-composition (oracle.vis.nearest_neighbor_within_patch on the device).  Needs a CUDA device.
+composition (oracle.vis.nearest_neighbor_within_patch on the device).
+Label propagation, N = 4, 512^2, 2 x 240 frames, a 256^2 label (65 536 points) at sigma 1.2: splat_composite_grid over all
+480 frames against the reference formulation (visualize_label_propagation: chunks of 100 (frame, image) pairs, two
+splat2d, the composite, .cpu(), then images2grid per frame on the host), timed over --label-chunks chunks and given per
+frame.  --labels-only runs this section alone.  Needs a CUDA device.
 """
 import argparse
 import os
@@ -26,7 +30,7 @@ from gangealing_b200.evaluation import congealing_average_frames  # noqa: E402
 from gangealing_b200.evaluation import visuals as V  # noqa: E402
 from gangealing_b200.stn import get_stn  # noqa: E402
 from gangealing_b200.stn.sampling import MipmapWarp, mipmap_warp_lerp_mean  # noqa: E402
-from gangealing_b200.splat2d import track_points_lerp  # noqa: E402
+from gangealing_b200.splat2d import splat2d, splat_composite_grid, track_points_lerp  # noqa: E402
 from oracle import opset  # noqa: E402
 from oracle import vis as OV  # noqa: E402
 
@@ -56,11 +60,59 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--frames-window", type=int, default=4)
     ap.add_argument("--n-mean", type=int, default=1000)
+    ap.add_argument("--label-chunks", type=int, default=2)
+    ap.add_argument("--labels-only", action="store_true")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("visbench: needs a CUDA device")
-    dev = "cuda"
     print("card: %s" % _card())
+    label_propagation(args.label_chunks)
+    if not args.labels_only:
+        congealing(args)
+
+
+def label_propagation(chunks):
+    """visualize_label_propagation's splat + grid loop against splat_composite_grid."""
+    from torchvision.utils import make_grid
+    dev, n, res, frames, side, batch = "cuda", 4, 512, 480, 256, 100
+    g = torch.Generator().manual_seed(1)
+    images = (torch.rand(frames, n, 3, res, res, generator=g) * 2 - 1).to(dev)
+    ys, xs = torch.meshgrid(torch.arange(side), torch.arange(side), indexing="ij")
+    label = (torch.stack([xs.flatten(), ys.flatten()], -1).float() * ((res - 1) / (side - 1))).to(dev)
+    drift = torch.randn(frames, n, 1, 2, generator=g).to(dev) * 20
+    points = (label.view(1, 1, -1, 2) + drift).contiguous()
+    p = label.size(0)
+    colors = (torch.rand(1, p, 3, generator=g) * 2 - 1).to(dev)
+    alpha = torch.rand(1, p, 1, generator=g).to(dev)
+    splat_composite_grid(images[:2], points[:2], colors, alpha, 1.2, 0.7, 2)
+    fused = _events(lambda: splat_composite_grid(images, points, colors, alpha, 1.2, 0.7, 2))
+    print("splat_composite_grid: N %d, %d^2, %d frames, %d points: %.1f ms per call = %.3f ms per frame" %
+          (n, res, frames, p, fused, fused / frames))
+
+    flat_images, flat_points = images.view(-1, 3, res, res), points.view(-1, p, 2)
+    col, al = colors.repeat(batch, 1, 1), alpha.repeat(batch, 1, 1)
+    sig = torch.full((batch,), 1.2, device=dev)
+
+    def reference(c):
+        sl = slice(c * batch, (c + 1) * batch)
+        obj = splat2d(torch.zeros(batch, 3, res, res, device=dev), flat_points[sl], col, sig, False)
+        mask = splat2d(torch.zeros(batch, 1, res, res, device=dev), flat_points[sl], al, sig, True) * 0.7
+        out = (mask * obj + (1 - mask) * flat_images[sl]).cpu().view(-1, n, 3, res, res)
+        return [make_grid(f, nrow=2, normalize=True, value_range=(-1, 1)).mul(255).add_(0.5).clamp_(0, 255)
+                .permute(1, 2, 0).to("cpu", torch.uint8).numpy() for f in out]
+
+    reference(0)
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    for c in range(chunks):
+        reference(c)
+    ref = (time.perf_counter() - t0) * 1e3 / (chunks * batch // n)
+    print("reference formulation (chunks of %d pairs: 2 splat2d + composite + .cpu() + images2grid per frame): %.2f ms per "
+          "frame (%d chunks); fused %.1fx" % (batch, ref, chunks, ref / (fused / frames)))
+
+
+def congealing(args):
+    dev = "cuda"
     res, batch, length = 512, 50, 240
     t = opset.fill_parameters(get_stn(["similarity", "flow"], flow_size=128, supersize=res, channel_multiplier=0.5).eval(),
                               51, gain=0.6).to(dev)

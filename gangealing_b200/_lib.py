@@ -89,6 +89,9 @@ SIGNATURES = {
     "gg_pck_transfer_workspace": (_L, [_L, _L, _I]),
     "gg_pck_transfer": (_I, [_P] * 14 + [_L, _L, _I, _I, _I, _I, _I, _P]),
     "gg_batch_gram": (_I, [_P, _P, _P, _P, _L, _I, _P]),
+    "gg_flow_image_grid": (_I, [_P, _P, _P, _L, _I, _I, _I, _I, _P]),
+    "gg_image_grid": (_I, [_P, _P, _P, _L, _I, _I, _I, _I, _P]),
+    "gg_cluster_accumulate": (_I, [_P] * 5 + [_L, _I, _I, _I, _I, _I] + [_L] * 6 + [_I, _P]),
 }
 
 _dll = None

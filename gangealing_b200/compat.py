@@ -11,6 +11,7 @@ It pre-registers, under the reference's module names, the modules that sit direc
   models.spatial_transformers.antialiased_sampling                  <- gangealing_b200.stn.sampling
   utils.splat2d_cuda (+ .functional, .splat)                        <- gangealing_b200.splat2d
   utils.laplacian_blending (LaplacianBlender)                       <- gangealing_b200.splat2d.blend
+  utils.vis_tools.flow_vis (flow_to_image)                          <- gangealing_b200.training.visuals
 so the reference never reaches its import-time JIT builds (`torch.utils.cpp_extension.load`, op/upfirdn2d.py:9-16,
 op/fused_act.py:10-17, utils/splat2d_cuda/functional.py:9-27 -- the last of which no longer compiles on modern
 torch).  Everything above those modules is the reference's own code, untouched.
@@ -50,4 +51,8 @@ def install(force=False):
     blend_mod = types.ModuleType("utils.laplacian_blending")     # the reference's needs cv2 for its 1-D Gaussians
     blend_mod.LaplacianBlender = _splat.LaplacianBlender
     register("utils.laplacian_blending", blend_mod)
+    from .training import visuals as _visuals
+    flow_vis = types.ModuleType("utils.vis_tools.flow_vis")       # train.py's flow images, colour wheel on the device
+    flow_vis.flow_to_image = _visuals.flow_to_image
+    register("utils.vis_tools.flow_vis", flow_vis)
     return pkg

@@ -26,6 +26,7 @@
 #include <algorithm>
 
 #include "common.cuh"
+#include "grid.cuh"
 #include "lookup.cuh"
 
 namespace gg {
@@ -136,7 +137,7 @@ splat_normalize_kernel(float* __restrict__ out, const float* __restrict__ input,
 struct GridParams {
   int64_t n, points;          // N images per frame, P points per image
   int r;                      // image side
-  int xmaps, pad, hg, wg;     // make_grid layout
+  GridLayout g;               // make_grid layout of one frame (grid.cuh)
   int colors_n, alpha_n;      // 1 (broadcast) or N
   float sigma, opacity;
 };
@@ -176,16 +177,6 @@ splat_frames_kernel(float* __restrict__ acc, const float* __restrict__ coords, c
   }
 }
 
-// make_grid's normalize (clamp(-1, 1), sub(-1), div(2)) and images2grid's mul(255), add(0.5), clamp(0, 255) and
-// truncating uint8 cast, each rounded on its own.
-__device__ __forceinline__ unsigned char quantise(float v) {
-  v = fminf(fmaxf(v, -1.f), 1.f);
-  v = __fdiv_rn(__fsub_rn(v, -1.f), 2.f);
-  v = __fadd_rn(__fmul_rn(v, 255.f), 0.5f);
-  v = fminf(fmaxf(v, 0.f), 255.f);
-  return static_cast<unsigned char>(static_cast<int>(v));
-}
-
 // One output pixel (3 bytes, HWC) of one frame's grid per thread.  SPLAT: composite the accumulated splats over the image
 // as splat2d's normalisation and splat_points' blend do, every operation rounded on its own:
 //   obj = S_c / (A + 1e-8);  m = (S_alpha / (max(A, 1) + 1e-8)) * opacity;  v = m * obj + (1 - m) * img.
@@ -196,16 +187,14 @@ composite_grid_kernel(unsigned char* __restrict__ out, const float* __restrict__
   constexpr int SLOTS = ALPHA ? 8 : 4;
   const int64_t idx = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (idx >= total) return;
-  const int gx = static_cast<int>(idx % p.wg);
-  const int64_t rest = idx / p.wg;
-  const int gy = static_cast<int>(rest % p.hg);
-  const int64_t frame = rest / p.hg;
+  const int gx = static_cast<int>(idx % p.g.wg);
+  const int64_t rest = idx / p.g.wg;
+  const int gy = static_cast<int>(rest % p.g.hg);
+  const int64_t frame = rest / p.g.hg;
   unsigned char* o = out + idx * 3;
-  const int cell = p.r + p.pad;
-  const int yy = gy - p.pad, xx = gx - p.pad;
-  const int y = yy >= 0 ? yy % cell : -1, x = xx >= 0 ? xx % cell : -1;
-  const int64_t k = yy >= 0 && xx >= 0 ? static_cast<int64_t>(yy / cell) * p.xmaps + xx / cell : -1;
-  if (y < 0 || y >= p.r || x < 0 || x >= p.r || k < 0 || k >= p.n) {   // make_grid's padding (pad value 0)
+  int y, x;
+  const int64_t k = grid_source(p.g, gx, gy, y, x);
+  if (k < 0) {   // make_grid's padding (pad value 0)
     o[0] = o[1] = o[2] = 0;
     return;
   }
@@ -224,9 +213,9 @@ composite_grid_kernel(unsigned char* __restrict__ out, const float* __restrict__
 #pragma unroll
     for (int c = 0; c < 3; ++c) v[c] = __fadd_rn(__fmul_rn(m, __fdiv_rn(sc[c], den)), __fmul_rn(keep, v[c]));
   }
-  o[0] = quantise(v[0]);
-  o[1] = quantise(v[1]);
-  o[2] = quantise(v[2]);
+  o[0] = quantise_range(v[0], -1.f, 1.f);   // images2grid: make_grid(normalize=True, range=(-1, 1))
+  o[1] = quantise_range(v[1], -1.f, 1.f);
+  o[2] = quantise_range(v[2], -1.f, 1.f);
 }
 
 inline int splat_grid(int64_t total, int threads) {
@@ -328,15 +317,12 @@ int gg_splat_composite_grid(unsigned char* out, void* workspace, int64_t workspa
     return fail(GG_ERR_BAD_ARG, "splat_composite_grid: points must be 8-byte aligned");
   GridParams p;
   p.n = N; p.points = P; p.r = R;
-  p.xmaps = static_cast<int>(N < nrow ? N : nrow);
-  const int64_t ymaps = (N + p.xmaps - 1) / p.xmaps;
-  p.pad = N == 1 ? 0 : padding;                      // make_grid returns a single image as it is
-  const int64_t hg = ymaps * (R + p.pad) + p.pad, wg = static_cast<int64_t>(p.xmaps) * (R + p.pad) + p.pad;
   const int slots = has_alpha ? 8 : 4;
   const int64_t frame_acc = N * R * static_cast<int64_t>(R) * slots;
-  if (hg * wg * 3 > kIntMax || frame_acc > kIntMax || N * 3 * R * static_cast<int64_t>(R) > kIntMax || N * P > kIntMax)
+  if (!make_grid_layout(p.g, N, R, R, nrow, padding) || frame_acc > kIntMax || N * 3 * R * static_cast<int64_t>(R) > kIntMax ||
+      N * P > kIntMax)
     return fail(GG_ERR_BAD_ARG, "splat_composite_grid: one frame's grid, images, accumulators or points exceed 2^31 elements");
-  p.hg = static_cast<int>(hg); p.wg = static_cast<int>(wg);
+  const int64_t hg = p.g.hg, wg = p.g.wg;
   p.colors_n = colors_n; p.alpha_n = alpha_n; p.sigma = sigma; p.opacity = opacity;
   const int64_t frame_bytes = frame_acc * static_cast<int64_t>(sizeof(float));
   // frames per launch: as many as the workspace holds, with every launch's thread count below 2^31

@@ -71,16 +71,21 @@ def _num_stages(t, vis_in_stages):
 
 @torch.no_grad()
 def average_congealed_image(t, loader, n_mean, classifier=None, cluster=None, num_heads=1, no_flip_inference=False,
-                            output_resolution=None, iters=1, padding_mode="border"):
-    """propagate_to_images.average + run_loader_mean(unfold=False) + utils/distributed.all_reduce: the mean of the
-    congealed (flipped) images of whole batches until this rank has seen at least n_mean // world images, over all ranks.
-    The sum is kept on the device instead of a host-side list of every congealed image.  -> (1, C, R, R)."""
+                            output_resolution=None, iters=1, padding_mode="border", unfold=False, keep=0):
+    """propagate_to_images.average + run_loader_mean + utils/distributed.all_reduce: the mean of the congealed (flipped)
+    images of whole batches until this rank has seen at least n_mean // world images, over all ranks.  The sum is kept
+    on the device instead of a host-side list of every congealed image.  -> (1, C, R, R).
+    unfold=True: every head congeals every image (the STN's (N, K, C, R, R) output) and the result is the per-head means
+    (K, C, R, R), as training_vis.run_loader_mean(unfold=True) returns them.  keep > 0: also return this rank's first
+    `keep` congealed images (the STN's output rows, in loader order) -> (mean, kept)."""
     world = dist.get_world_size()
-    acc, total = None, 0
+    acc, total, kept = None, 0, []
     for x in loader:
         flipped, _, policy = _flips(t, x, classifier, cluster, num_heads, no_flip_inference, iters, padding_mode)
-        out = t(flipped, warp_policy=policy, unfold=False, iters=iters, padding_mode=padding_mode,
+        out = t(flipped, warp_policy=policy, unfold=unfold, iters=iters, padding_mode=padding_mode,
                 output_resolution=output_resolution)
+        if sum(k.size(0) for k in kept) < keep:
+            kept.append(out[:keep - sum(k.size(0) for k in kept)])
         s = out.float().sum(dim=0, keepdim=True)
         acc = s if acc is None else acc + s
         total += x.size(0)
@@ -89,7 +94,8 @@ def average_congealed_image(t, loader, n_mean, classifier=None, cluster=None, nu
     if acc is None:
         raise ValueError("average_congealed_image: the loader yielded no images")
     num = dist.all_gather(torch.tensor([float(total)], device=acc.device)).sum()
-    return dist.all_gather(acc).sum(dim=0, keepdim=True) / num
+    mean = dist.all_gather(acc).sum(dim=0, keepdim=not unfold) / num
+    return (mean, torch.cat(kept, 0)) if keep > 0 else mean
 
 
 @torch.no_grad()

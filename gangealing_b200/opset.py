@@ -27,6 +27,7 @@ def cuda_ops():
         from .op import vgg_pool as _vp
         from .evaluation import ops as _ev
         from .op import pca as _pca
+        from .op import grids as _grids
         _cached = types.SimpleNamespace(
             name="sm_90a",
             upfirdn2d=_op.upfirdn2d,
@@ -59,5 +60,8 @@ def cuda_ops():
             mipmap_warp_lerp_mean=_smp.mipmap_warp_lerp_mean,   # ... and their per-frame batch sums, frames never written
             track_points_lerp=_track_points_lerp,         # dense point tracking over a stage's frames, one launch
             splat_composite_grid=_splat_composite_grid,   # label propagation: splats + composite + uint8 grid per frame
+            flow_image_grid=_grids.flow_image_grid,       # training visuals: colour-wheel flow images as a uint8 grid
+            image_grid=_grids.image_grid,                 # ... min/max-normalised uint8 grid (per-image ranges)
+            cluster_accumulate=_grids.cluster_accumulate,  # ... per-cluster sums of routed images, in order, on the device
         )
     return _cached

@@ -557,6 +557,37 @@ GG_API int gg_scale_cast_multi(const void* table, const int* block_tensor, const
 GG_API int gg_batch_gram(double* gram, double* mean, const float* w, const int64_t* batch_offsets, int64_t B, int D,
                          void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Training visuals, csrc/trainvis.cu (reference utils/vis_tools/training_vis.py, flow_vis.py).  Grids are uint8 (Hg, Wg, 3)
+ * in torchvision make_grid's layout (nrow, padding, pad value 0, xmaps = min(nrow, N); N == 1: the bare image), the layout
+ * gg_splat_composite_grid writes.  Arguments are validated before any device work (GG_ERR_BAD_ARG).
+ *   gg_flow_image_grid: flow_to_image (flow_vis.py:106-130, flow_uv_to_colors :70-103) of flow (N, H, W, 2) fp32, 8-byte
+ *     aligned, written as the grid.  u, v = flow * (H - 1); the radius maximum over the whole batch (np.max(rad), one
+ *     reduction, atomicMax on the float bits: order-independent); numpy's precision as the reference runs it: float32 up
+ *     to fk = (atan2(-v, -u) / pi + 1) / 2 * 54, float64 from f = fk - k0 on.  The value written is floor(255 * col): the
+ *     reference's / 255, make_grid(range=(0, 1)) and * 255 + 0.5 return exactly that.  workspace: 4 bytes, 8-byte aligned.
+ *   gg_image_grid: make_grid(normalize=True) with per-image ranges + images2grid (helpers.py:39-43): images (N, 3, H, W)
+ *     fp32 dense; ranges (N, 2) fp32 (lo, hi), 8-byte aligned; clamp(lo, hi), sub(lo), div(max(hi - lo, 1e-5)), * 255,
+ *     + 0.5, clamp(0, 255), truncation, every operation rounded on its own.  range=None, scale_each=True: each image's
+ *     (min, max); a value_range: the same (lo, hi) for every image.
+ *   gg_cluster_accumulate: routes congealed images to clusters (generate_cluster_congeal / real_cluster_congeal,
+ *     training_vis.py:57-109).  Image n, slot s = sel[n] in [0, S): the element (c, y, x) of image n, flip s / K, head s % K
+ *     is read at images + n*stride_n + (s/K)*stride_flip + (s%K)*stride_head + c*stride_c + y*stride_h + x*stride_w (so
+ *     assign_fake_images_to_clusters' (2, N, K, C, H, W) output is passed as it is; a (N, C, H, W) batch with
+ *     stride_flip = stride_head = 0).  It is added to sums[s % K] (K, C, H, W) fp32, counts[s % K] (K,) int64 is
+ *     incremented, and while counts[s % K] < n_keep the image is copied to keep[s % K, counts[s % K]] (K, n_keep, C, H, W).
+ *     Each sum element adds its images one by one in n order (no atomics): across calls, bitwise the sequential fp32 sum.
+ *     sums, counts and keep carry over from call to call; the caller zeroes them first.  Entries outside [0, S) are skipped.
+ * ---------------------------------------------------------------------------------------------- */
+GG_API int gg_flow_image_grid(unsigned char* out, void* workspace, const float* flow, int64_t N, int H, int W, int nrow,
+                              int padding, void* stream);
+GG_API int gg_image_grid(unsigned char* out, const float* images, const float* ranges, int64_t N, int H, int W, int nrow,
+                         int padding, void* stream);
+GG_API int gg_cluster_accumulate(float* sums, int64_t* counts, float* keep, const float* images, const int64_t* sel,
+                                 int64_t N, int S, int K, int C, int H, int W, int64_t stride_n, int64_t stride_flip,
+                                 int64_t stride_head, int64_t stride_c, int64_t stride_h, int64_t stride_w, int n_keep,
+                                 void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -316,8 +316,8 @@ def bilinear_downsample(input, stride, kernel_horz, kernel_vert):
     separable tent filter with stride, as ONE gather kernel (csrc/resample.cu).  Half-precision images are filtered in
     fp32 and cast back; there is no ATen route."""
     _lib.require_cuda(input)
-    if input.dim() != 4 or 2 * stride > 32:
-        raise RuntimeError("bilinear_downsample: expected a (N, C, H, W) image and stride <= 16, got %s, stride %d" %
+    if input.dim() != 4 or not 1 <= stride <= 16:
+        raise RuntimeError("bilinear_downsample: expected a (N, C, H, W) image and stride in 1..16, got %s, stride %d" %
                            (tuple(input.shape), stride))
     channels = input.shape[1]
     taps = 2 * stride

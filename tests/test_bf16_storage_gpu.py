@@ -17,14 +17,13 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from fp64_contract import DEV, SQRT2, blur_plan, ceil_div, finish_depth, lrelu64, randn, rowwise_c, seeded, slope_gain
 from oracle import stylegan2_ops as so
 from oracle.rounding import assert_fp32_sum, assert_rounded_once
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda"
 CL = torch.channels_last
 BF = torch.bfloat16
-SQRT2 = 2 ** 0.5
 CS = [64, 192, 512]                   # 192: a non-power-of-two multiple of the bf16 blur multiple (64)
 SPATIAL = [(4, 4), (9, 9), (33, 29)]
 
@@ -39,25 +38,8 @@ def check_sum(y, ref, a, c, what, extra=None):
     print("[contract] %s: c_obs=%.2f (c=%d)" % (what, r, c))
 
 
-def _gen(seed):
-    return torch.Generator(device=DEV).manual_seed(seed)
-
-
-def randn(*shape, g, dtype=torch.float32):
-    return torch.randn(*shape, generator=g, device=DEV).to(dtype)
-
-
 def cl(t):
     return t.contiguous(memory_format=CL)
-
-
-def lrelu64(t, slope, gain):
-    return torch.where(t > 0, t, t * slope) * gain
-
-
-def slope_gain(slope, gain):
-    """Leaky-ReLU and gain scale |pre-activation| by at most this."""
-    return abs(gain) * max(1.0, abs(slope))
 
 
 def fir64(x, k, pad):
@@ -77,44 +59,6 @@ def fir64(x, k, pad):
 def _sm():
     from gangealing_b200 import _lib
     return _lib.sm_count()
-
-
-def _ceil(a, b):
-    return -(-a // b)
-
-
-def finish_depth(k):
-    """nhwc_finish_kernel: a lane's serial chain over every 32nd of the K partial rows, (a0 + a1) + (a2 + a3), then the 32
-    lane sums in order."""
-    return _ceil(k, 32) + 2 + 32
-
-
-def rowwise_geometry(n, cv, hw, sms=None):
-    """rowwise_chunk / bwd_chunk of csrc/nhwc.cu, csrc/styled.cu for C/V = cv channel vectors, planned for `sms` SMs (default:
-    this device's): (pixel lanes, pixels per CTA, CTAs per sample)."""
-    lanes = max(256 // cv, 1)
-    k = max(1, min(_ceil(8 * (sms or _sm()), n), _ceil(hw, 4 * lanes)))
-    chunk = _ceil(hw, k)
-    return lanes, chunk, _ceil(hw, chunk)
-
-
-def rowwise_c(n, c, hw, per_term, per_sample, v=8, sms=None):
-    """A thread's serial sum over its pixels, the CTA's pixel lanes in order, then the finish kernel over the CTAs.
-    v: channels per 16-byte vector (8 bf16, 4 fp32)."""
-    lanes, chunk, k = rowwise_geometry(n, c // v, hw, sms)
-    return per_term + _ceil(chunk, lanes) + lanes + finish_depth(k if per_sample else n * k)
-
-
-def blur_geometry(n, c, out_h, out_w):
-    """blur_plan of csrc/nhwc.cu (bf16: 32 output columns, 64 channels per CTA): (rows per segment, CTAs per sample and
-    channel chunk)."""
-    xblocks = _ceil(out_w, 32)
-    segs = _ceil(4 * _sm(), xblocks * (c // 64) * n)
-    seg_rows = _ceil(out_h, segs)
-    if seg_rows < 16:
-        seg_rows = out_h if out_h < 16 else 16
-    seg_rows = _ceil(seg_rows, 4) * 4
-    return seg_rows, xblocks * _ceil(out_h, seg_rows)
 
 
 def blur_k(kernel):
@@ -139,12 +83,12 @@ def filt(kind, gain=1.0):
 def test_noise_bias_act_nhwc(c, hw, noise, row_scale):
     """o = lrelu(rs*x + b + nw*noise)*gain: nw*noise, the fma, + noise, *slope, *gain -> k = 5."""
     from gangealing_b200.op import nhwc
-    g = _gen(c + hw[0])
+    g = seeded(c + hw[0])
     n = 3
-    x = cl(randn(n, c, *hw, g=g, dtype=BF))
-    nz = randn(n, 1, *hw, g=g) if noise else None
+    x = cl(randn((n, c, *hw), g, BF))
+    nz = randn((n, 1, *hw), g) if noise else None
     nw = torch.tensor([0.7], device=DEV) if noise else None
-    b = randn(c, g=g)
+    b = randn((c,), g)
     rs = torch.rand(n, c, generator=g, device=DEV) + 0.5 if row_scale else None
     y = nhwc.noise_bias_act(x, nz, nw, b, rs, 0.2, SQRT2)
     x64 = x.double()
@@ -164,16 +108,16 @@ def test_bias_act_backward_nhwc(c, hw):
     from gangealing_b200.op import nhwc
     if hw == (257, 257) and c != 192:
         pytest.skip("one channel count at the full-size plane")
-    g = _gen(c * 7 + hw[0])
+    g = seeded(c * 7 + hw[0])
     n = 2
-    gy = cl(randn(n, c, *hw, g=g, dtype=BF))
-    out = randn(n, c, *hw, g=g)
+    gy = cl(randn((n, c, *hw), g, BF))
+    out = randn((n, c, *hw), g)
     out = cl(torch.where(torch.rand(out.shape, generator=g, device=DEV) < 0.05, torch.zeros_like(out), out).to(BF))
     gx, gb = nhwc.bias_act_backward(gy, out, 0.2, SQRT2, True)
     slope = torch.where(out.double() > 0, 1.0, 0.2) * SQRT2
     ref = gy.double() * slope
     check_once(gx, ref, ref.abs(), 2, "bias_act_backward gx C=%d %s" % (c, hw))
-    check_sum(gb, ref.sum((0, 2, 3)), ref.abs().sum((0, 2, 3)), rowwise_c(n, c, hw[0] * hw[1], 2, False),
+    check_sum(gb, ref.sum((0, 2, 3)), ref.abs().sum((0, 2, 3)), rowwise_c(n, c, hw[0] * hw[1], 2, False, BF, _sm()),
               "bias_act_backward grad_bias C=%d %s" % (c, hw))
 
 
@@ -182,16 +126,16 @@ def test_bias_act_backward_nhwc(c, hw):
 def test_channel_scale_with_row_dot_nhwc(c, hw):
     """out = x*s (k = 1); row_dot = sum_p x*y (one fma per pixel on a thread's chain)."""
     from gangealing_b200.op import nhwc
-    g = _gen(c * 3 + hw[1])
+    g = seeded(c * 3 + hw[1])
     n = 3
-    x = cl(randn(n, c, *hw, g=g, dtype=BF))
-    yv = cl(randn(n, c, *hw, g=g, dtype=BF))
-    s = randn(n, c, g=g)
+    x = cl(randn((n, c, *hw), g, BF))
+    yv = cl(randn((n, c, *hw), g, BF))
+    s = randn((n, c), g)
     out, dot = nhwc.channel_scale(x, s, yv)
     ref = x.double() * s.double()[:, :, None, None]
     check_once(out, ref, ref.abs(), 1, "channel_scale C=%d %s" % (c, hw))
     t = x.double() * yv.double()
-    check_sum(dot, t.sum((2, 3)), t.abs().sum((2, 3)), rowwise_c(n, c, hw[0] * hw[1], 0, True),
+    check_sum(dot, t.sum((2, 3)), t.abs().sum((2, 3)), rowwise_c(n, c, hw[0] * hw[1], 0, True, BF, _sm()),
               "channel_scale row_dot C=%d %s" % (c, hw))
 
 
@@ -203,9 +147,9 @@ def test_channel_scale_with_row_dot_nhwc(c, hw):
 def test_blur_mode0_nhwc(c, hw, pad, gain, kind):
     """Plain blur (the STN trunk's pads (1,1) / (2,2)): k = blur_k."""
     from gangealing_b200.op import nhwc
-    g = _gen(c + hw[0] + pad)
+    g = seeded(c + hw[0] + pad)
     k = filt(kind, gain)
-    x = cl(randn(2, c, *hw, g=g, dtype=BF))
+    x = cl(randn((2, c, *hw), g, BF))
     p4 = (pad, pad, pad, pad)
     y, _, _ = nhwc.blur(x, k, p4, mode=0)
     check_once(y, fir64(x.double(), k, p4), fir64(x.double().abs(), k.abs(), p4), blur_k(k),
@@ -225,16 +169,16 @@ def test_blur_mode1_fused_tail_nhwc(shape, slope, kind):
     if shape[2] == 257 and (kind != "sep" or slope != 0.2):
         pytest.skip("the benchmark layer in its own configuration")
     n, c, h, w = shape
-    g = _gen(c + h + int(slope * 10))
+    g = seeded(c + h + int(slope * 10))
     k = filt(kind, 4.0)
     p4 = (1, 1, 1, 1)
-    x = cl(randn(n, c, h, w, g=g, dtype=BF))
+    x = cl(randn((n, c, h, w), g, BF))
     oh, ow = h - 1, w - 1
-    nz = randn(n, 1, oh, ow, g=g)
+    nz = randn((n, 1, oh, ow), g)
     nw = torch.tensor([0.3], device=DEV)
-    b = randn(c, g=g) * 0.5
+    b = randn((c,), g) * 0.5
     rs = torch.rand(n, c, generator=g, device=DEV) + 0.5
-    s2 = randn(n, c, g=g) + 1.0
+    s2 = randn((n, c), g) + 1.0
     out, out2, _ = nhwc.blur(x, k, p4, mode=1, noise=nz, noise_weight=nw, bias=b, row_scale=rs, scale2=s2, want_out=True,
                              want_out2=True, negative_slope=slope, gain=SQRT2)
     r64, s64 = rs.double()[:, :, None, None], s2.double()[:, :, None, None]
@@ -257,21 +201,21 @@ def test_blur_mode2_adjoint_epilogue_nhwc(shape, kind):
     if shape[2] == 256 and kind != "sep":
         pytest.skip("the benchmark layer with its own filter")
     n, c, h, w = shape
-    g = _gen(c + h + 5)
+    g = seeded(c + h + 5)
     k = torch.flip(filt(kind, 4.0), [0, 1]).contiguous()
     p4 = (2, 2, 2, 2)                                  # the adjoint of the (1, 1)-padded 4-tap blur
-    x = cl(randn(n, c, h, w, g=g, dtype=BF))
+    x = cl(randn((n, c, h, w), g, BF))
     oh, ow = h + 1, w + 1
     rs = torch.rand(n, c, generator=g, device=DEV) + 0.5
-    mul = cl(randn(n, c, oh, ow, g=g, dtype=BF))
+    mul = cl(randn((n, c, oh, ow), g, BF))
     y, _, dot = nhwc.blur(x, k, p4, mode=2, row_scale=rs, mul=mul, want_dot=True)
     t, ta = fir64(x.double(), k, p4), fir64(x.double().abs(), k.abs(), p4)
     r64 = rs.double()[:, :, None, None]
     what = "blur mode 2 %s %s" % (kind, tuple(shape))
     check_once(y, t * r64, ta * r64, blur_k(k) + 1, what + " g_raw")
-    seg_rows, kc = blur_geometry(n, c, oh, ow)
+    p = blur_plan(BF, n, c, h, w, 4, 4, p4, _sm())
     check_sum(dot, (t * mul.double()).sum((2, 3)), (ta * mul.double().abs()).sum((2, 3)),
-              blur_k(k) + 1 + seg_rows + 32 + finish_depth(kc), what + " dot")
+              blur_k(k) + 1 + p["seg_rows"] + 32 + finish_depth(p["xblocks"] * p["segs"]), what + " dot")
 
 
 TAIL_SHAPES = [(3, 64, 4, 4), (2, 192, 9, 9), (2, 512, 33, 29), (2, 128, 256, 256)]
@@ -279,11 +223,11 @@ TAIL_SHAPES = [(3, 64, 4, 4), (2, 192, 9, 9), (2, 512, 33, 29), (2, 128, 256, 25
 
 def tail_inputs(shape, seed):
     n, c, h, w = shape
-    g = _gen(seed)
-    t = {"raw": cl(randn(n, c, h, w, g=g, dtype=BF)), "noise": randn(n, 1, h, w, g=g), "nw": torch.tensor([0.3], device=DEV),
-         "bias": randn(c, g=g) * 0.5, "demod": torch.rand(n, c, generator=g, device=DEV) + 0.5,
-         "s_next": randn(n, c, g=g) + 1.0, "wm": randn(n, 3, c, g=g) / c ** 0.5, "rgb_bias": randn(3, g=g),
-         "skip": randn(n, 3, h, w, g=g)}
+    g = seeded(seed)
+    t = {"raw": cl(randn((n, c, h, w), g, BF)), "noise": randn((n, 1, h, w), g), "nw": torch.tensor([0.3], device=DEV),
+         "bias": randn((c,), g) * 0.5, "demod": torch.rand(n, c, generator=g, device=DEV) + 0.5,
+         "s_next": randn((n, c), g) + 1.0, "wm": randn((n, 3, c), g) / c ** 0.5, "rgb_bias": randn((3,), g),
+         "skip": randn((n, 3, h, w), g)}
     return t
 
 
@@ -322,10 +266,10 @@ def test_styled_tail_backward_nhwc(shape, slope):
     from gangealing_b200.op import nhwc
     n, c, h, w = shape
     t = tail_inputs(shape, c + h + 1)
-    g = _gen(c + h + 2)
-    gxs = cl(randn(n, c, h, w, g=g, dtype=BF))
-    grgb = randn(n, 3, h, w, g=g)
-    out = randn(n, c, h, w, g=g)
+    g = seeded(c + h + 2)
+    gxs = cl(randn((n, c, h, w), g, BF))
+    grgb = randn((n, 3, h, w), g)
+    out = randn((n, c, h, w), g)
     out = cl(torch.where(torch.rand(out.shape, generator=g, device=DEV) < 0.05, torch.zeros_like(out), out).to(BF))
     g_raw, d_s, d_d, d_w = nhwc.styled_tail_backward(gxs, grgb, out, t["raw"], t["s_next"], t["demod"], t["wm"], True, True,
                                                      True, slope, SQRT2)
@@ -338,7 +282,7 @@ def test_styled_tail_backward_nhwc(shape, slope):
     gt, gta = go * sl, goa * sl.abs()
     what = "styled_tail_backward slope %g %s" % (slope, tuple(shape))
     check_once(g_raw, gt * d64, gta * d64.abs(), 7, what + " g_raw")
-    c0 = rowwise_c(n, c, h * w, 0, True)
+    c0 = rowwise_c(n, c, h * w, 0, True, BF, _sm())
     o64, r64 = out.double(), t["raw"].double()
     check_sum(d_s, (gxs.double() * o64).sum((2, 3)), (gxs.double() * o64).abs().sum((2, 3)), c0, what + " d_s_next")
     check_sum(d_d, (gt * r64).sum((2, 3)), (gta * r64.abs()).sum((2, 3)), c0 + 6, what + " d_demod")
@@ -363,9 +307,9 @@ def distance_forward_c(n, c, hw):
     the warp sum (5), the CTA's 8 warps, *1/HW (2), the finish kernel's K partials."""
     s, e_ia, trips, L = distance_c_terms(c)
     groups = 256 // L
-    k = max(1, min(_ceil(8 * _sm(), n), _ceil(hw, 2 * groups), 64))
-    chunk = _ceil(hw, k)
-    return int(math.ceil(2 * (e_ia + 2) + 4 * trips + _ceil(chunk, groups) + 5 + 8 + 2 + _ceil(hw, chunk)))
+    k = max(1, min(ceil_div(8 * _sm(), n), ceil_div(hw, 2 * groups), 64))
+    chunk = ceil_div(hw, k)
+    return int(math.ceil(2 * (e_ia + 2) + 4 * trips + ceil_div(chunk, groups) + 5 + 8 + 2 + ceil_div(hw, chunk)))
 
 
 def distance_backward_k(c):
@@ -406,12 +350,12 @@ def distance64(a, b, w, gout, eps=1e-10):
 def test_feature_distance_bf16_value_and_gradients(c, weighted, stacked):
     """Every <L, TRIPS> instantiation of launch_distance (L = 1..32, TRIPS = 1, 2, 3, 4, 6, 8), forward and backward."""
     from gangealing_b200.op.feature_distance import feature_distance, feature_distance_stacked
-    g = _gen(c + 2 * int(weighted) + int(stacked))
+    g = seeded(c + 2 * int(weighted) + int(stacked))
     n, h, w = 2, 6, 5
-    a = cl(torch.relu(randn(n, c, h, w, g=g)).to(BF))
-    b = cl(torch.relu(randn(n, c, h, w, g=g) + 0.2).to(BF))
+    a = cl(torch.relu(randn((n, c, h, w), g)).to(BF))
+    b = cl(torch.relu(randn((n, c, h, w), g) + 0.2).to(BF))
     wt = torch.rand(c, generator=g, device=DEV) + 0.1 if weighted else None
-    gout = randn(n, 1, 1, 1, g=g)
+    gout = randn((n, 1, 1, 1), g)
     if stacked:
         f = cl(torch.cat([a, b])).requires_grad_(True)
         r = feature_distance_stacked(f, wt)
@@ -436,11 +380,11 @@ def test_bias_relu_pool_bf16_forward_and_backward(shape):
     (k = 1) with the arg-max decided on the stored y."""
     from gangealing_b200.op.vgg_pool import bias_relu_pool
     n, c, h, w = shape
-    g = _gen(c + h)
-    raw = cl(randn(*shape, g=g, dtype=BF)).requires_grad_(True)
-    bias = randn(c, g=g)
-    gy = cl(randn(*shape, g=g, dtype=BF))
-    gp = cl(randn(n, c, h // 2, w // 2, g=g, dtype=BF))
+    g = seeded(c + h)
+    raw = cl(randn(shape, g, BF)).requires_grad_(True)
+    bias = randn((c,), g)
+    gy = cl(randn(shape, g, BF))
+    gp = cl(randn((n, c, h // 2, w // 2), g, BF))
     y, p = bias_relu_pool(raw, bias)
     pre = raw.detach().double() + bias.double()[:, None, None]
     check_once(y, torch.relu(pre), raw.detach().double().abs() + bias.double().abs()[:, None, None], 1,
@@ -463,11 +407,11 @@ def test_weight_scaler_bf16_products_are_rounded_once():
     as one fp32 value -> k = 2.  Sizes cover several 32768-element chunks, a tail that is not a multiple of 4, and two
     tensors in one launch."""
     from gangealing_b200.op.scaled_weights import WeightScaler
-    g = _gen(5)
+    g = seeded(5)
     mods = [torch.nn.Linear(1, 1, bias=False).to(DEV) for _ in range(3)]
     sizes = [(512, 300), (3, 7, 5), (64, 3, 3, 3)]
     for m, sz in zip(mods, sizes):
-        m.weight = torch.nn.Parameter(randn(*sz, g=g))
+        m.weight = torch.nn.Parameter(randn(sz, g))
     scales = [1 / math.sqrt(300), 1 / math.sqrt(35), 1 / math.sqrt(27)]
     gains = [1.0, SQRT2, 1.0]
     scaler = WeightScaler(list(zip(mods, scales)))
@@ -502,7 +446,7 @@ def nchw_k(kernel):
 def nchw_sum_c(m):
     """An fp32 reduction of m terms on the NCHW kernels: a thread's serial chain (at most m/32 terms), warp and CTA sums
     (5 + 8), a finish chain over the partials (at most m/32 + 5): bounded by 2*ceil(m/32) + 20."""
-    return 2 * _ceil(m, 32) + 20
+    return 2 * ceil_div(m, 32) + 20
 
 
 @pytest.mark.parametrize("dtype", HALF)
@@ -510,9 +454,9 @@ def nchw_sum_c(m):
 @pytest.mark.parametrize("kind", ["sep", "rand"])
 def test_upfirdn2d_nchw_half(dtype, shape, kind):
     from gangealing_b200 import op
-    g = _gen(shape[2] + shape[3])
+    g = seeded(shape[2] + shape[3])
     k = _nchw_filter(kind)
-    x = randn(*shape, g=g, dtype=dtype)
+    x = randn(shape, g, dtype)
     y = op.upfirdn2d(x, k, pad=(1, 1))
     p4 = (1, 1, 1, 1)
     check_once(y, fir64(x.double(), k, p4), fir64(x.double().abs(), k.abs(), p4), nchw_k(k),
@@ -526,12 +470,12 @@ def test_blur_noise_bias_act_nchw_half(dtype, shape):
     k = blur_k + the fma with rs, the fma with the noise, slope*gain, the product -> blur_k + 4."""
     from gangealing_b200 import op
     n, c, h, w = shape
-    g = _gen(h + w + 1)
+    g = seeded(h + w + 1)
     k = _nchw_filter("sep")
-    x = randn(*shape, g=g, dtype=dtype)
-    nz = randn(n, 1, h - 1, w - 1, g=g, dtype=dtype)
+    x = randn(shape, g, dtype)
+    nz = randn((n, 1, h - 1, w - 1), g, dtype)
     nw = torch.tensor([0.3], device=DEV)
-    b = randn(c, g=g) * 0.5
+    b = randn((c,), g) * 0.5
     rs = torch.rand(n, c, generator=g, device=DEV) + 0.5
     y = op.blur_noise_bias_act(x, k, (1, 1), nz, nw, b, row_scale=rs)
     p4 = (1, 1, 1, 1)
@@ -551,10 +495,10 @@ def test_elementwise_nchw_half(dtype, shape):
     from gangealing_b200 import op
     from gangealing_b200.op.modconv import channel_scale_raw
     n, c, h, w = shape
-    g = _gen(h * w + c)
-    x = randn(*shape, g=g, dtype=dtype)
-    b = randn(c, g=g)
-    gy = randn(*shape, g=g, dtype=dtype)
+    g = seeded(h * w + c)
+    x = randn(shape, g, dtype)
+    b = randn((c,), g)
+    gy = randn(shape, g, dtype)
     what = "%s %s" % (dtype, shape)
     xl, bl = x.clone().requires_grad_(True), b.clone().requires_grad_(True)
     y = op.fused_leaky_relu(xl, bl)
@@ -568,7 +512,7 @@ def test_elementwise_nchw_half(dtype, shape):
     check_sum(gb, gx.double().sum((0, 2, 3)), gx.double().abs().sum((0, 2, 3)), nchw_sum_c(n * h * w),
               "fused_leaky_relu grad_bias " + what)
     # noise + bias + leaky-ReLU with a row scale
-    nz = randn(n, 1, h, w, g=g, dtype=dtype)
+    nz = randn((n, 1, h, w), g, dtype)
     nw = torch.tensor([0.7], device=DEV)
     rs = torch.rand(n, c, generator=g, device=DEV) + 0.5
     y = op.noise_bias_act(x, nz, nw, b, row_scale=rs)
@@ -578,7 +522,7 @@ def test_elementwise_nchw_half(dtype, shape):
     a = ((x.double() * r64).abs() + b.double().abs()[:, None, None] + noise.abs()) * slope_gain(0.2, SQRT2)
     check_once(y, lrelu64(pre, 0.2, SQRT2), a, 5, "noise_bias_act " + what)
     # channel scale with its row dot
-    s = randn(n, c, g=g)
+    s = randn((n, c), g)
     out, dot = channel_scale_raw(x, s, y=gy)
     ref = x.double() * s.double()[:, :, None, None]
     check_once(out, ref, ref.abs(), 1, "channel_scale " + what)

@@ -12,9 +12,10 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from demod_reference import demod_inputs
+from fp64_contract import grid_stride_batch
 from oracle import flow as FL
 from oracle import sampling as S
-from test_sampling_gpu import grid_stride_batch
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -84,7 +85,6 @@ def test_flow_compose_gradients_are_deterministic():
 
 def test_demodulation_is_deterministic():
     """The demodulation coefficients (single-layer and batched launches) and their style gradients."""
-    from test_demod_precision import demod_inputs
     from gangealing_b200.op import style_path
     from gangealing_b200.op.modconv import demod_coefficients
     w, s, scale = demod_inputs(65, 200, 257)

@@ -21,27 +21,20 @@ path when it finishes.
 """
 import math
 import re
-from collections import defaultdict
 
 import numpy as np
 import pytest
 import torch
 
+from fp64_contract import (DEV, F32, H100_SMS, SQRT2, Worst, assert_routes_reached, at_offset, blur_plan, ceil_div,
+                           launched, seeded)
 from oracle import stylegan2_ops as so
-from oracle.rounding import assert_fp32_sum
 
-DEV = "cuda"
-SQRT2 = 2 ** 0.5
 GG_F32 = 0                        # gangealing_b200._lib.GG_F32
-H100_SMS = 132                    # SM count the CPU coverage check plans the NHWC grid with (H100 SXM)
 
 # ======================================================================================== planner restatement (no GPU)
 K_RS, K_CO, K_WARPS, K_GUARD, K_MAX_PPI = 8, 4, 8, 16, 32   # csrc/upfirdn2d.cu band-kernel constants
 STAGE_BUDGET, RING_LIMIT = 36 * 1024, 64 * 1024
-
-
-def _ceil(a, b):
-    return -(-a // b)
 
 
 def out_size(h, w, kh, kw, up, down, pad):
@@ -64,29 +57,29 @@ def band_plan(planes, in_h, in_w, out_h, out_w, pad_x0, es=4):
     strips_x = out_w // strip_w if out_w // strip_w > 0 else 1
 
     def slot(rows):
-        rows8 = _ceil(rows, K_RS) * K_RS
-        return _ceil(K_GUARD // es + (rows8 + 3) * in_w + 2 * per16 + 4, per16) * per16
+        rows8 = ceil_div(rows, K_RS) * K_RS
+        return ceil_div(K_GUARD // es + (rows8 + 3) * in_w + 2 * per16 + 4, per16) * per16
 
     ppi = 1
     if slot(out_h) * es <= STAGE_BUDGET:
         r, bands = out_h, 1
-        tasks = strips_x * _ceil(out_h, strip_h)
-        ppi = min(_ceil(K_WARPS, tasks), STAGE_BUDGET // (slot(out_h) * es))
+        tasks = strips_x * ceil_div(out_h, strip_h)
+        ppi = min(ceil_div(K_WARPS, tasks), STAGE_BUDGET // (slot(out_h) * es))
         ppi = min(max(ppi, 1), planes, K_MAX_PPI)
     else:
-        r = strip_h * _ceil(K_WARPS, strips_x)
+        r = strip_h * ceil_div(K_WARPS, strips_x)
         while r > strip_h and slot(r) * es > STAGE_BUDGET:
             r -= strip_h
         if slot(r) * es > RING_LIMIT:
             return None, "ring"
         if r >= out_h:
             return None, "one band"
-        bands = _ceil(out_h, r)
+        bands = ceil_div(out_h, r)
     if slot(r) * ppi * es * 3 > 200 * 1024:
         return None, "smem"
     return dict(planes=planes, in_h=in_h, in_w=in_w, out_h=out_h, out_w=out_w, pad_x0=pad_x0, lx_log2=lx_log2, r=r,
                 bands=bands, ppi=ppi, slot=slot(r), slot_of=slot, es=es,
-                n_items=_ceil(planes, ppi) if bands == 1 else planes * bands), None
+                n_items=ceil_div(planes, ppi) if bands == 1 else planes * bands), None
 
 
 def band_walk(p, pad_y0, in_off):
@@ -110,10 +103,10 @@ def band_walk(p, pad_y0, in_off):
         lo = max(vy0, 0)
         nreal = min(vy0 + vrows - 1, in_h - 1) - lo + 1
         n_top = (lo if nreal > 0 else vy0 + vrows) - vy0
-        d0 = _ceil(K_GUARD // 4 + n_top * in_w, 4) * 4
+        d0 = ceil_div(K_GUARD // 4 + n_top * in_w, 4) * 4
         geom = dict(m0=m0, n_planes=n_planes, oy0=oy0, rows=rows, nreal=nreal)
-        main_tasks = full_x * _ceil(rows, (32 >> p["lx_log2"]) * K_RS)
-        tail_tasks = _ceil(rows, (32 >> lt) * K_RS) if tail_w > 0 else 0
+        main_tasks = full_x * ceil_div(rows, (32 >> p["lx_log2"]) * K_RS)
+        tail_tasks = ceil_div(rows, (32 >> lt) * K_RS) if tail_w > 0 else 0
         for pl in range(n_planes):
             if nreal <= 0:
                 v0 = d0 - vrows * in_w
@@ -231,22 +224,10 @@ def _threshold_labels(plan, why, out_h, out_w, in_w):
     return lab
 
 
-def nhwc_plan(n, c, in_h, in_w, kh, kw, pad, sms):
-    """blur_plan of csrc/nhwc.cu for fp32 storage (32 channels and 64 output columns per CTA)."""
-    out_h, out_w = in_h + pad[2] + pad[3] - kh + 1, in_w + pad[0] + pad[1] - kw + 1
-    xblocks, chunks = _ceil(out_w, 64), c // 32
-    segs = _ceil(4 * sms, xblocks * chunks * n)
-    seg_rows = _ceil(out_h, segs)
-    if seg_rows < 16:
-        seg_rows = out_h if out_h < 16 else 16
-    seg_rows = _ceil(seg_rows, 4) * 4
-    return dict(out_h=out_h, out_w=out_w, xblocks=xblocks, chunks=chunks, seg_rows=seg_rows, segs=_ceil(out_h, seg_rows))
-
-
 def nhwc_route(shape, k, pad, mode, slope, gain, sms):
     n, c, h, w = shape
     sep, e = band_factor(k)
-    p = nhwc_plan(n, c, h, w, k.shape[0], k.shape[1], pad, sms)
+    p = blur_plan(F32, n, c, h, w, k.shape[0], k.shape[1], pad, sms)
     fast = mode == 1 and gain > 0 and 0 <= slope <= 1
     name = "blur_nhwc_kernel<float, %d, %s, %s>" % (mode, str(sep).lower(), str(fast).lower())
     labels = {name}
@@ -427,11 +408,7 @@ def test_cases_reach_every_fp32_fir_path():
     reached = set()
     for r in all_routes():
         reached |= r["labels"]
-    missing = [lab for lab in REQUIRED if lab not in reached]
-    print("[coverage] %d of %d fp32 FIR classes reached" % (len(REQUIRED) - len(missing), len(REQUIRED)))
-    for lab in REQUIRED:
-        print("[coverage]   %s %s" % ("ok     " if lab in reached else "MISSING", lab))
-    assert not missing, "fp32 FIR classes no case reaches: %s" % missing
+    assert_routes_reached(REQUIRED, reached, noun="fp32 FIR classes")
 
 
 def test_wide_pads_leave_the_band_kernel_and_hot_pads_stay():
@@ -448,34 +425,13 @@ def test_wide_pads_leave_the_band_kernel_and_hot_pads_stay():
 
 
 # ======================================================================================================== GPU checks
-WORST = defaultdict(float)
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _report_worst():
-    yield
-    if WORST:
-        print("\n[contract] worst observed c per fp32 FIR path:")
-        for path in sorted(WORST):
-            print("[contract]   %-46s c_obs = %.2f" % (path, WORST[path]))
-
-
-def check_sum(y, ref, a, c, path, what, extra=None):
-    r = assert_fp32_sum(y, ref, a, c, "%s: %s" % (path, what), extra)
-    WORST[path] = max(WORST[path], r)
-    print("[contract] %s: %s: c_obs=%.2f (c=%d)" % (path, what, r, c))
+WORST = Worst("c per fp32 FIR path", "%-46s c_obs = %.2f", kind_suffix=False)
+_report_worst = WORST.fixture()
+check_sum = WORST.check_sum
 
 
 def ref64(x, k, up=(1, 1), down=(1, 1), pad=(0, 0, 0, 0)):
     return so.upfirdn2d_ref_full(x.double(), k.to(x.device).double(), up[0], up[1], down[0], down[1], *pad)
-
-
-def at_offset(t, off):
-    """A copy of `t` whose data starts `off` elements past a 16-byte boundary (torch allocations are 512-byte aligned)."""
-    buf = torch.empty(off + t.numel(), dtype=t.dtype, device=t.device)
-    v = buf[off:].view(t.shape)
-    v.copy_(t)
-    return v
 
 
 def fir_raw(x, k, up=(1, 1), down=(1, 1), pad=(0, 0, 0, 0), out_off=0):
@@ -504,10 +460,6 @@ def fused_raw(x, k, pad, noise, nw, bias, rs, act, alpha, scale, out_off=0):
     return out
 
 
-def _gen(seed):
-    return torch.Generator(device=DEV).manual_seed(seed)
-
-
 def check_fir(y, x, k, route, what, up=(1, 1), down=(1, 1), pad=(0, 0, 0, 0)):
     """y = upfirdn2d(x, k): every element within c * 2^-24 * sum|x*k| of the float64 value (+ the factorisation error)."""
     kd = k.to(DEV)
@@ -520,7 +472,7 @@ def check_fir(y, x, k, route, what, up=(1, 1), down=(1, 1), pad=(0, 0, 0, 0)):
 def test_band_strip_variant(w, px0, fused, vec):
     """One launch per StripF32<IW4, *, FUSED, VEC> x pad_x0: the item's plane alignments supply every S0."""
     cs = strip_case(w, px0, fused, vec)
-    g = _gen(w * 8 + px0)
+    g = seeded(w * 8 + px0)
     x = at_offset(torch.randn(cs["shape"], generator=g, device=DEV), cs["in_off"])
     k = cs["k"].to(DEV)
     pad = cs["pad"]
@@ -571,7 +523,7 @@ def test_filters_and_pads_forward_and_backward(fi, pi):
     flipped filter, grad_pad) against the float64 adjoint."""
     from gangealing_b200.op.upfirdn2d import UpFirDn2d
     cs = sweep_case(fi, pi)
-    g = _gen(100 * fi + pi)
+    g = seeded(100 * fi + pi)
     k = cs["k"].to(DEV)
     x = torch.randn(cs["shape"], generator=g, device=DEV).requires_grad_(True)
     y = UpFirDn2d.apply(x, k, (1, 1), (1, 1), cs["pad"])
@@ -588,7 +540,7 @@ def test_filters_and_pads_forward_and_backward(fi, pi):
 @pytest.mark.parametrize("case", range(len(GEOMETRY_CASES)))
 def test_band_geometry_and_thresholds(case):
     shape, pad = GEOMETRY_CASES[case]
-    g = _gen(7 + case)
+    g = seeded(7 + case)
     k = filt("binom") if case % 2 == 0 else filt("full")
     x = torch.randn(shape, generator=g, device=DEV)
     route = fir_route(shape, k, pad=pad)
@@ -600,7 +552,7 @@ def test_band_geometry_and_thresholds(case):
 def test_polyphase_resamplers_and_fallbacks(case):
     """x2 up-sampler: 4 fmas per output (c = 4); x2 decimator: 16 (c = 16); the generic fallback: kh*kw."""
     shape, up, down, pad, io, oo = POLY_CASES[case]
-    g = _gen(50 + case)
+    g = seeded(50 + case)
     k = filt("binom") if case % 2 == 0 else filt("full")
     x = at_offset(torch.randn(shape, generator=g, device=DEV), io)
     route = fir_route(shape, k, (up, up), (down, down), pad, io, oo)
@@ -613,7 +565,7 @@ def test_polyphase_resamplers_and_fallbacks(case):
 def test_polyphase_autograd(up):
     """The to-RGB skip's Upsample and its backward (each resampler is the other's adjoint), through autograd."""
     from gangealing_b200 import op
-    g = _gen(up)
+    g = seeded(up)
     k = filt("binom").to(DEV)
     down = 3 - up
     pad = (2, 1) if up == 2 else (1, 1)
@@ -635,7 +587,7 @@ def test_blur_noise_bias_act_epilogue(nz, b, rs, e):
     cs = tail_case(nz, b, rs, e)
     act, slope, gain = cs["epi"]
     n, c, h, w = cs["shape"]
-    g = _gen(1000 + 16 * nz + 8 * b + 4 * rs + e)
+    g = seeded(1000 + 16 * nz + 8 * b + 4 * rs + e)
     x = torch.randn(cs["shape"], generator=g, device=DEV)
     k = cs["k"].to(DEV)
     oh, ow = out_size(h, w, 4, 4, (1, 1), (1, 1), cs["pad"])
@@ -653,7 +605,7 @@ def test_blur_noise_bias_act_epilogue(nz, b, rs, e):
 def nhwc_dot_c(route):
     p = route["plan"]
     # mode 2's dot: a thread's fmas over its 2 columns x segment rows, the CTA's 32 column groups, the finish kernel
-    return route["c"] + 1 + 2 * p["seg_rows"] + 32 + (_ceil(p["xblocks"] * p["segs"], 32) + 2 + 32)
+    return route["c"] + 1 + 2 * p["seg_rows"] + 32 + (ceil_div(p["xblocks"] * p["segs"], 32) + 2 + 32)
 
 
 @pytest.mark.gpu
@@ -666,7 +618,7 @@ def test_blur_nhwc_f32(si, mode, kind, ep):
     slope, gain = ep
     shape, pad = NHWC_SHAPES[si], NHWC_PADS[si]
     n, c, h, w = shape
-    g = _gen(300 + 10 * si + mode)
+    g = seeded(300 + 10 * si + mode)
     k = filt(kind, seed=si)
     kd = k.to(DEV)
     route = nhwc_route(shape, k, pad, mode, slope, gain, _lib.sm_count())
@@ -706,15 +658,7 @@ def test_blur_nhwc_f32(si, mode, kind, ep):
                   what + " row_dot", (fx * m64.abs()).sum((2, 3)) if fx is not None else None)
 
 
-def launched(fn):
-    """Names of the project's FIR kernels `fn` launches, from torch.profiler's CUDA activity."""
-    from torch.profiler import ProfilerActivity, profile
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        fn()
-        torch.cuda.synchronize()
-    pat = re.compile(r"(fir4_band_kernel|upfirdn2d_generic_kernel|up2_k4_kernel|down2_k4_kernel|blur_nhwc_kernel)(<[^>]*>)?")
-    return [m.group(0) for e in prof.events() for m in [pat.search(e.name)] if m]
+KERNELS = re.compile(r"(fir4_band_kernel|upfirdn2d_generic_kernel|up2_k4_kernel|down2_k4_kernel|blur_nhwc_kernel)(<[^>]*>)?")
 
 
 def routing_cases():
@@ -759,9 +703,9 @@ def test_routing_matches_the_restatement():
             oh, ow = out_size(shape[2], shape[3], *k.shape, up, down, pad)
             nz, nw = torch.randn(n, oh, ow, device=DEV), torch.ones(1, device=DEV)
             b, rs = torch.zeros(c, device=DEV), torch.ones(n * c, device=DEV)
-            names = launched(lambda: fused_raw(x, kd, pad, nz, nw, b, rs, 3, 0.2, SQRT2, oo))
+            names = launched(lambda: fused_raw(x, kd, pad, nz, nw, b, rs, 3, 0.2, SQRT2, oo), KERNELS)
         else:
-            names = launched(lambda: fir_raw(x, kd, up, down, pad, oo))
+            names = launched(lambda: fir_raw(x, kd, up, down, pad, oo), KERNELS)
         seen.append("%-48s -> %s" % (label, names))
         assert names == [route["name"]], "%s: launched %s, the restatement predicts %s" % (label, names, route["name"])
     for si, mode, kind, (slope, gain) in NHWC_CASES:
@@ -778,7 +722,7 @@ def test_routing_matches_the_restatement():
             kwargs = dict(row_scale=torch.ones(shape[0], shape[1], device=DEV), want_dot=True,
                           mul=torch.ones(shape[0], shape[1], p["out_h"], p["out_w"], device=DEV).contiguous(
                               memory_format=torch.channels_last))
-        names = [nm for nm in launched(lambda: nhwc.blur(x, kd, pad, mode=mode, **kwargs))]
+        names = [nm for nm in launched(lambda: nhwc.blur(x, kd, pad, mode=mode, **kwargs), KERNELS)]
         seen.append("%-48s -> %s" % ("nhwc %s mode %d %s slope %g" % (shape, mode, kind, slope), names))
         assert names == [route["name"]], (shape, mode, kind, names, route["name"])
     for line in seen:
@@ -802,7 +746,7 @@ def test_zero_weight_columns_stay_finite_after_nan_in_shared_memory():
     def poison():
         assert bool(torch.isnan(fir_raw(nan_x, k4.to(DEV), pad=(1, 1, 1, 1))).all())
 
-    g = _gen(77)
+    g = seeded(77)
     for shape, (kh, kw), pad in WIDE_PAD_CASES:
         k = k4 if kh == 4 else filt("full", kh, kw)
         x = torch.randn(shape, generator=g, device=DEV)

@@ -32,28 +32,21 @@ Every check prints its worst observed c (`[contract] ...` lines with `pytest -s`
 path when it finishes.
 """
 import math
-from collections import defaultdict
 
 import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
+from fp64_contract import BF16, DEV, F16, F32, H100_SMS, Worst, assert_routes_reached, grid_for, library, seeded
 from oracle.rounding import U32, assert_fp32_sum, assert_rounded_once
 from oracle.sampling import create_stack, downsample_2x, grid_sample_bilinear
 
-DEV = "cuda"
-H100_SMS = 132
 THREADS = 256
 MAX_LEVELS = 8                                  # warp.cu kMaxLevels
 STATIC_SMEM, OPTIN_SMEM = 48 * 1024, 200 * 1024
-F32, F16, BF16 = torch.float32, torch.float16, torch.bfloat16
 SHORT = {F32: "f32", F16: "f16", BF16: "bf16"}
 PAD_MODES = ("zeros", "border", "reflection")
-
-
-def _ceil(a, b):
-    return -(-a // b)
 
 
 # ======================================================================================== planner restatement (no GPU)
@@ -102,11 +95,6 @@ def pyramid_elems(planes, hs, ws, extra):
 
 def level_shape(py, i):
     return py["hp"] >> i, py["wp"] >> i
-
-
-def grid_for(total, threads=THREADS, sms=H100_SMS):
-    """flow_compose.cuh grid_for: enough CTAs for `total` items, at most 16 per SM (grid-stride beyond that)."""
-    return min(max(_ceil(total, threads), 1), 16 * sms)
 
 
 def _trips(tag, total, sms):
@@ -275,11 +263,7 @@ def test_cases_reach_every_route():
     width's padding, one and several grid-stride trips of the level-1 launches, single-level reads at every L = 0..8 by
     both mechanisms, and for the tent every stride 1..16 at its smallest legal plane and one row / column more."""
     reached = all_labels()
-    missing = [lab for lab in REQUIRED if lab not in reached]
-    print("[coverage] %d of %d routes reached" % (len(REQUIRED) - len(missing), len(REQUIRED)))
-    for lab in REQUIRED:
-        print("[coverage]   %s %s" % ("ok     " if lab in reached else "MISSING", lab))
-    assert not missing, "routes no case reaches: %s" % missing
+    assert_routes_reached(REQUIRED, reached)
 
 
 def test_every_case_is_feasible_and_routed_as_labelled():
@@ -344,16 +328,8 @@ def test_restated_tent_legality_matches_the_entry():
 
 
 # ======================================================================================================== GPU checks
-WORST = defaultdict(float)
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _report_worst():
-    yield
-    if WORST:
-        print("\n[contract] worst observed c per path:")
-        for path in sorted(WORST):
-            print("[contract]   %-48s %.2f" % (path, WORST[path]))
+WORST = Worst("c per path", "%-48s %.2f")
+_report_worst = WORST.fixture()
 
 
 def check(y, ref, a, c, path, what):
@@ -362,17 +338,8 @@ def check(y, ref, a, c, path, what):
         _, obs = assert_rounded_once(y, ref, a, c, "%s: %s" % (path, what))
     else:
         obs = assert_fp32_sum(y, ref, a, c, "%s: %s" % (path, what))
-    WORST[path] = max(WORST[path], obs)
+    WORST.note(path, obs)
     print("[contract] %s: %s: obs=%.2f (bound %g)" % (path, what, obs, c))
-
-
-def _lib():
-    from gangealing_b200 import _lib as lib
-    return lib
-
-
-def _gen(seed):
-    return torch.Generator(device=DEV).manual_seed(seed)
 
 
 def pyramid64(x64, py, extra):
@@ -417,7 +384,7 @@ def test_pyramid_levels(case):
     planes, hs, ws, extra, dtype = case
     py = make_pyramid(hs, ws, planes, extra)
     route = build_route(planes, hs, ws, extra)
-    x = torch.randn(1, planes, hs, ws, generator=_gen(hs * 7 + ws + extra), device=DEV).to(dtype)
+    x = torch.randn(1, planes, hs, ws, generator=seeded(hs * 7 + ws + extra), device=DEV).to(dtype)
     flat = _pyramid(x, extra)
     assert flat.numel() == py["offsets"][0]
     x64 = x[0].double().cpu()
@@ -473,10 +440,10 @@ def test_pyramid_adjoint(case):
     """gg_mipmap_build_backward adds build^T(G) to grad_src and leaves every intermediate level holding its own total
     gradient; compared per level with the float64 transpose, and by <build(x), G> = <x, build^T(G)> in float64."""
     from gangealing_b200.stn.sampling import _pyramid
-    lib = _lib()
+    lib = library()
     planes, hs, ws, extra = case
     py = make_pyramid(hs, ws, planes, extra)
-    gen = _gen(hs * 13 + ws + extra)
+    gen = seeded(hs * 13 + ws + extra)
     G = [torch.randn(planes, hs, ws, generator=gen, device=DEV)]
     G += [torch.randn(planes, *level_shape(py, i), generator=gen, device=DEV) for i in range(1, extra + 1)]
     grad_pyr = torch.cat([g.reshape(-1) for g in G[1:]])
@@ -518,13 +485,13 @@ def test_pyramid_adjoint(case):
     assert abs(lhs - rhs) <= bound, "inner-product identity: |%.9g - %.9g| > %.3g" % (lhs, rhs, bound)
     print("[contract] adjoint identity: P%d-%dx%d-E%d: |<Px, G> - <x, P^T G>| = %.3g <= %.3g" %
           (planes, hs, ws, extra, abs(lhs - rhs), bound))
-    WORST["adjoint identity (in units of the grad_src c)"] = max(WORST["adjoint identity (in units of the grad_src c)"], obs)
+    WORST.note("adjoint identity (in units of the grad_src c)", obs)
 
 
 @pytest.mark.gpu
 def test_pyramid_adjoint_without_work_leaves_grad_src_untouched():
-    lib = _lib()
-    gen = _gen(5)
+    lib = library()
+    gen = seeded(5)
     grad_src = torch.randn(3, 64, 64, generator=gen, device=DEV)
     grad_pyr = torch.randn(3 * 32 * 32, generator=gen, device=DEV)
     keep_src, keep_pyr = grad_src.clone(), grad_pyr.clone()
@@ -565,9 +532,9 @@ def test_single_level_reads(case):
     level L (oracle/sampling.py create_stack: the level upsampled to the padded size, cropped by lp), for every L = 0..E
     and every padding mode, with no pixel exempt."""
     from gangealing_b200.stn.sampling import _pyramid
-    lib = _lib()
+    lib = library()
     n, c, hs, ws, extra, dtype = case
-    x = torch.randn(n, c, hs, ws, generator=_gen(hs * 3 + ws), device=DEV).to(dtype)
+    x = torch.randn(n, c, hs, ws, generator=seeded(hs * 3 + ws), device=DEV).to(dtype)
     pyr = _pyramid(x, extra)
     x64 = x.double().cpu()
     stack, stack_abs = create_stack(x64, extra + 1), create_stack(x64.abs(), extra + 1)
@@ -614,7 +581,7 @@ def test_tent_forward_and_adjoint(case):
     backward against float64, and <T x, g> = <x, T^T g>."""
     from gangealing_b200.stn.sampling import bilinear_downsample
     n, c, h, w, s = case
-    gen = _gen(h * 100 + w + s)
+    gen = seeded(h * 100 + w + s)
     x = torch.randn(n, c, h, w, generator=gen, device=DEV)
     kh = torch.randn(c, 2 * s, generator=gen, device=DEV)
     kv = torch.randn(c, 2 * s, generator=gen, device=DEV)
@@ -647,7 +614,7 @@ def test_tent_entries_refuse_bad_strides_and_planes():
     """The Python face raises on a stride outside 1..16 and on a plane not larger than s // 2, and the entries refuse
     them on real tensors, leaving the output as it was."""
     from gangealing_b200.stn.sampling import bilinear_downsample
-    lib = _lib()
+    lib = library()
     x = torch.randn(1, 3, 8, 8, device=DEV)
     for s in (0, 17):
         with pytest.raises(RuntimeError):

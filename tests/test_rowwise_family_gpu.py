@@ -28,28 +28,13 @@ elements and the NHWC 64-bit index path at more than 2^32 vectors), which need 8
 """
 import math
 import re
-from collections import defaultdict
 
-import numpy as np
 import pytest
 import torch
 
-from oracle.rounding import assert_fp32_sum, assert_rounded_once
-from test_bf16_storage_gpu import finish_depth, rowwise_c, rowwise_geometry
-from test_fir_fp32_gpu import at_offset
-
-DEV = "cuda"
-SQRT2 = 2 ** 0.5
-H100_SMS = 132                    # SM count the CPU coverage check plans with (H100 SXM)
-F32, F16, BF16 = torch.float32, torch.float16, torch.bfloat16
-VEC = {F32: 4, F16: 8, BF16: 8}   # elements per 16-byte access
-TNAME = {F32: "float", F16: "__half", BF16: "__nv_bfloat16"}
-CODE = {F32: 0, F16: 1, BF16: 2}  # gangealing_b200._lib.GG_F32 / GG_F16 / GG_BF16
-SHORT = {F32: "fp32", F16: "fp16", BF16: "bf16"}
-
-
-def _ceil(a, b):
-    return -(-a // b)
+from fp64_contract import (BF16, CODE, DEV, F16, F32, H100_SMS, SHORT, SQRT2, TNAME, VEC, Worst, assert_routes_reached,
+                           at_offset, ceil_div, f32, finish_depth, launched, library, lrelu64, nan_at, randn, rowwise_c,
+                           rowwise_geometry, saved_output, seeded, slope_gain)
 
 
 # ======================================================================================== planner restatement (no GPU)
@@ -58,7 +43,7 @@ def row_geom(mode, hw):
     if hw < 1024:
         return True, hw, 1
     chunk = 16384 if mode == 0 else 8192
-    return False, chunk, _ceil(hw, chunk)
+    return False, chunk, ceil_div(hw, chunk)
 
 
 def nchw_rowwise_route(dtype, mode, n, c, hw, want_sum=True, x_off=0, y_off=0, out_off=0):
@@ -72,7 +57,7 @@ def nchw_rowwise_route(dtype, mode, n, c, hw, want_sum=True, x_off=0, y_off=0, o
     labels = set()
     if small:
         names = ["rowwise_nchw_rows_kernel<%s, %d>" % (tn, mode)]
-        chain, cta = _ceil(hw, 32), 0
+        chain, cta = ceil_div(hw, 32), 0
         labels.add("%s: rows, N*C %s" % (tag, "a multiple of 8" if rows % 8 == 0 else "not a multiple of 8"))
     else:
         shape_ok = hw % v == 0
@@ -80,7 +65,7 @@ def nchw_rowwise_route(dtype, mode, n, c, hw, want_sum=True, x_off=0, y_off=0, o
         vec = shape_ok and aligned
         names = ["rowwise_nchw_kernel<%s, %d, %d>" % (tn, v if vec else 1, mode)]
         m = min(chunk, hw)
-        chain, cta = (_ceil(m, 256 * v) * v if vec else _ceil(m, 256)), 8
+        chain, cta = (ceil_div(m, 256 * v) * v if vec else ceil_div(m, 256)), 8
         labels.add("%s: %s" % (tag, "vector" if vec else "scalar (shape)" if not shape_ok else
                                "scalar (x misaligned)" if x_off % v else "scalar (y misaligned)" if y_off % v else
                                "scalar (out misaligned)"))
@@ -99,7 +84,7 @@ def nchw_rowwise_route(dtype, mode, n, c, hw, want_sum=True, x_off=0, y_off=0, o
     if want_sum:
         if mode == 1:
             names.append("bias_grad_finish_kernel")
-            finish = _ceil(n * k, 32) + 5
+            finish = ceil_div(n * k, 32) + 5
         elif not small:
             names.append("row_finish_kernel")
             finish = k
@@ -161,9 +146,9 @@ def nhwc_rowwise_route(dtype, n, c, hw, sms=H100_SMS):
 
 def to_rgb_route(n, c, hw, sms=H100_SMS):
     """gg_to_rgb_nhwc_forward's chunking (a multiple of the 128 pixels one trip covers) and the backward's rowwise_chunk."""
-    k = max(1, min(_ceil(8 * sms, n), _ceil(hw, 128)))
-    chunk = _ceil(_ceil(hw, k), 128) * 128
-    kf = _ceil(hw, chunk)
+    k = max(1, min(ceil_div(8 * sms, n), ceil_div(hw, 128)))
+    chunk = ceil_div(ceil_div(hw, k), 128) * 128
+    kf = ceil_div(hw, chunk)
     labels = {"to_rgb_nhwc_fwd_kernel", "to_rgb_nhwc_bwd_kernel", "to-RGB fwd: K %s" % ("= 1" if kf == 1 else "> 1"),
               "to-RGB fwd: %s" % ("float4 stores (HW % 4 == 0)" if hw % 4 == 0 else "scalar stores (HW % 4 != 0)")}
     if hw % 128:
@@ -270,7 +255,7 @@ def nhwc_cases(sms=H100_SMS):
         for cv in NHWC_CVS:
             lanes = max(256 // cv, 1)
             c = cv * VEC[dt]
-            k5 = _ceil(8 * sms, 5)
+            k5 = ceil_div(8 * sms, 5)
             out += [(dt, 1, c, 4 * lanes - 1), (dt, 5, c, 4 * lanes + 1), (dt, 5, c, k5 * 5 * lanes + 3)]
     return out
 
@@ -359,13 +344,7 @@ def test_cases_reach_every_route():
     reached = set()
     for r in all_routes():
         reached |= r["labels"]
-    missing = [lab for lab in REQUIRED if lab not in reached]
-    print("[coverage] %d of %d routes reached" % (len(REQUIRED) - len(missing), len(REQUIRED)))
-    for lab in REQUIRED:
-        print("[coverage]   %s %s" % ("ok     " if lab in reached else "MISSING", lab))
-    for lab in UNREACHED:
-        print("[coverage]   unreached (8-16 GB tensors) %s" % lab)
-    assert not missing, "routes no case reaches: %s" % missing
+    assert_routes_reached(REQUIRED, reached, ["(8-16 GB tensors) " + lab for lab in UNREACHED])
 
 
 def test_restated_geometry_matches_the_workspace_queries():
@@ -382,66 +361,10 @@ def test_restated_geometry_matches_the_workspace_queries():
 
 
 # ======================================================================================================== GPU checks
-WORST = defaultdict(float)
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _report_worst():
-    yield
-    if WORST:
-        print("\n[contract] worst observed k (stored values) / c (sums) per route:")
-        for path in sorted(WORST):
-            print("[contract]   %-64s %.2f" % (path, WORST[path]))
-
-
-def check_stored(y, ref, a, k, path, what):
-    """A stored value: fp32 within k * 2^-24 * A; fp16 / bf16 within 1/2 ulp + k * 2^-24 * A."""
-    if y.dtype == F32:
-        obs = assert_fp32_sum(y, ref, a, k, "%s: %s" % (path, what))
-    else:
-        _, obs = assert_rounded_once(y, ref, a, k, "%s: %s" % (path, what))
-    WORST[path + " (k)"] = max(WORST[path + " (k)"], obs)
-    print("[contract] %s: %s: k_obs=%.2f (k=%d)" % (path, what, obs, k))
-
-
-def check_sum(y, ref, a, c, path, what):
-    obs = assert_fp32_sum(y, ref, a, c, "%s: %s" % (path, what))
-    WORST[path + " (c)"] = max(WORST[path + " (c)"], obs)
-    print("[contract] %s: %s: c_obs=%.2f (c=%d)" % (path, what, obs, c))
-
-
-def _gen(seed):
-    return torch.Generator(device=DEV).manual_seed(seed)
-
-
-def randn(shape, g, dtype=F32, off=0):
-    t = torch.randn(shape, generator=g, device=DEV).to(dtype)
-    return at_offset(t, off) if off else t
-
-
-def saved_output(shape, g, dtype, off=0):
-    """A forward output to gate on: mixed signs and ~5 % exact zeros (zero takes the negative slope)."""
-    t = torch.randn(shape, generator=g, device=DEV)
-    t = torch.where(torch.rand(shape, generator=g, device=DEV) < 0.05, torch.zeros_like(t), t).to(dtype)
-    return at_offset(t, off) if off else t
-
-
-def nan_at(shape, dtype, off=0):
-    """An output buffer `off` elements past a 16-byte boundary, filled with NaN: an element no launch writes stays NaN."""
-    buf = torch.full((off + math.prod(shape),), float("nan"), dtype=dtype, device=DEV)
-    return buf[off:].view(shape)
-
-
-def f32(v):
-    """A Python float as the fp32 value a kernel argument holds."""
-    return float(np.float32(v))
-
-
+WORST = Worst("k (stored values) / c (sums) per route")
+_report_worst = WORST.fixture()
+check_stored, check_sum = WORST.check_stored, WORST.check_sum
 A32, G32 = f32(0.2), f32(SQRT2)       # the slope and gain as the launches receive them
-
-
-def lrelu64(t, slope, gain):
-    return torch.where(t > 0, t, t * f32(slope)) * f32(gain)
 
 
 def act_grad64(gate):
@@ -450,20 +373,11 @@ def act_grad64(gate):
     return torch.where(gate > 0, torch.ones_like(gate), torch.full_like(gate, A32)) * G32
 
 
-def slope_gain(slope, gain):
-    return abs(gain) * max(1.0, abs(slope))
-
-
-def _lib():
-    from gangealing_b200 import _lib as lib
-    return lib
-
-
 # ---------------------------------------------------------------------------------------------- NCHW row-wise
 def nchw_rowwise(case, g):
     """Runs one NCHW_CASES entry through the C ABI -> (out, sum or None, x, y, s)."""
     dt, mode, n, c, hw, want_sum, xo, yo, oo = case
-    L = _lib()
+    L = library()
     lib = L.load()
     x = randn((n, c, hw), g, dt, xo)
     out = nan_at((n, c, hw), dt, oo)
@@ -493,7 +407,7 @@ def test_rowwise_nchw(case):
     dt, mode, n, c, hw, want_sum, xo, yo, oo = case
     route = nchw_rowwise_route(dt, mode, n, c, hw, want_sum, xo, yo, oo)
     path = route["names"][0]
-    out, sm, x, y, s = nchw_rowwise(case, _gen(hw + 31 * mode + 7 * xo + 3 * yo))
+    out, sm, x, y, s = nchw_rowwise(case, seeded(hw + 31 * mode + 7 * xo + 3 * yo))
     x64 = x.double()
     if mode == 0:
         ref = x64 * s.double().reshape(n, c, 1)
@@ -513,7 +427,7 @@ def test_rowwise_nchw(case):
 # ---------------------------------------------------------------------------------------------- flat kernel
 def flat_run(case, g):
     dt, shape, layout, act, grad, b, xo, ro = case
-    L = _lib()
+    L = library()
     c = shape[1]
     x = randn(shape, g, dt, xo)
     bias = torch.randn(c, generator=g, device=DEV) if b else None
@@ -540,7 +454,7 @@ def test_flat_bias_act(case):
     as fused_bias_act_raw does); grad = 2 stores exact zeros."""
     dt, shape, layout, act, grad, b, xo, ro = case
     route = flat_route(dt, math.prod(shape), flat_step(shape, layout), b, grad == 1, xo, ro)
-    out, x, bias, ref = flat_run(case, _gen(act * 10 + grad + 100 * xo + 1000 * ro + len(shape)))
+    out, x, bias, ref = flat_run(case, seeded(act * 10 + grad + 100 * xo + 1000 * ro + len(shape)))
     path = route["names"][0]
     if grad == 2:
         assert bool((out == 0).all()), "%s: grad = 2 must store zeros" % path
@@ -553,13 +467,13 @@ def test_flat_bias_act(case):
         r64 = pre * G32
     else:
         gate = pre if grad == 0 else ref.double()
-        r64 = lrelu64(pre, 0.2, SQRT2) if grad == 0 else torch.where(gate > 0, pre, pre * A32) * G32
+        r64 = lrelu64(pre, A32, G32) if grad == 0 else torch.where(gate > 0, pre, pre * A32) * G32
     check_stored(out, r64, a, 3, path, "act %d grad %d %s %s" % (act, grad, layout, tuple(shape)))
 
 
 # ---------------------------------------------------------------------------------------------- noise_bias_act NCHW
 def noise_run(dt, shape, nz, nw, b, rs, xo, no, g):
-    L = _lib()
+    L = library()
     n, c, h, w = shape
     hw = h * w
     x = randn((n, c, hw), g, dt, xo)
@@ -578,7 +492,7 @@ def noise_run(dt, shape, nz, nw, b, rs, xo, no, g):
     if nz:
         t = (0.7 if nw else 1.0) * noise.double()[:, None, :]
         pre, a = pre + t, a + t.abs()
-    return out, lrelu64(pre, 0.2, SQRT2), a * slope_gain(0.2, SQRT2)
+    return out, lrelu64(pre, A32, G32), a * slope_gain(0.2, SQRT2)
 
 
 @pytest.mark.gpu
@@ -588,8 +502,8 @@ def test_noise_bias_act_nchw(case):
     """out = RN(lrelu(rs*x + b + nw*noise)*gain): the fma with rs, the noise fma, *slope, *gain and one more for the scalar
     kernel's separate product -> k = 5.  noise_weight = None means 1."""
     dt, shape, nz, nw, b, rs, xo, no = case
-    route = noise_route(dt, shape[0], shape[1], shape[2] * shape[3], nz, xo, no, _lib().sm_count())
-    out, ref, a = noise_run(dt, shape, nz, nw, b, rs, xo, no, _gen(sum(shape) + 2 * nz + 4 * nw + 8 * b + 16 * rs))
+    route = noise_route(dt, shape[0], shape[1], shape[2] * shape[3], nz, xo, no, library().sm_count())
+    out, ref, a = noise_run(dt, shape, nz, nw, b, rs, xo, no, seeded(sum(shape) + 2 * nz + 4 * nw + 8 * b + 16 * rs))
     check_stored(out, ref, a, 5, route["names"][0], "%s noise %s nw %s bias %s rs %s" % (shape, nz, nw, b, rs))
 
 
@@ -597,11 +511,11 @@ def test_noise_bias_act_nchw(case):
 @pytest.mark.parametrize("dt", HALF_ALL)
 def test_noise_bias_act_scalar_grid_stride(dt):
     """A scalar-route tensor larger than 16 CTAs x 256 threads per SM: threads take a second grid-stride trip."""
-    sms = _lib().sm_count()
+    sms = library().sm_count()
     n, c, hw = big_scalar_shape(sms)
     route = noise_route(dt, n, c, hw, True, sms=sms)
     assert "noise nchw: scalar, a second grid-stride trip" in route["labels"]
-    out, ref, a = noise_run(dt, (n, c, hw, 1), True, False, True, True, 0, 0, _gen(5))
+    out, ref, a = noise_run(dt, (n, c, hw, 1), True, False, True, True, 0, 0, seeded(5))
     check_stored(out, ref, a, 5, route["names"][0], "grid-stride (%d, %d, %d)" % (n, c, hw))
 
 
@@ -624,11 +538,10 @@ def test_rowwise_nhwc(case):
     pixel lanes in order, nhwc_finish_kernel over the CTAs (per sample for row_dot, over N*K for grad_bias)."""
     from gangealing_b200.op import nhwc
     dt, n, c, hw = case
-    sms = _lib().sm_count()
+    sms = library().sm_count()
     route = nhwc_rowwise_route(dt, n, c, hw, sms)
     shape = nhwc_shape(n, c, hw)
-    g = _gen(c + hw + n)
-    v = VEC[dt]
+    g = seeded(c + hw + n)
     what = "C=%d HW=%d N=%d (lanes %d, chunk %d, K %d)" % (c, hw, n, route["lanes"], route["chunk"], route["k"])
     x, y = cl(randn(shape, g, dt)), cl(randn(shape, g, dt))
     s = torch.randn(n, c, generator=g, device=DEV)
@@ -636,13 +549,13 @@ def test_rowwise_nhwc(case):
     ref = x.double() * s.double()[:, :, None, None]
     check_stored(out, ref, ref.abs(), 1, route["names"][0][0], what + " out")
     t = x.double() * y.double()
-    check_sum(dot, t.sum((2, 3)), t.abs().sum((2, 3)), rowwise_c(n, c, hw, 0, True, v, sms), route["names"][0][0],
+    check_sum(dot, t.sum((2, 3)), t.abs().sum((2, 3)), rowwise_c(n, c, hw, 0, True, dt, sms), route["names"][0][0],
               what + " row_dot")
     saved = cl(saved_output(shape, g, dt))
     gx, gb = nhwc.bias_act_backward(x, saved, 0.2, SQRT2, True)
     ref = x.double() * act_grad64(saved.double())
     check_stored(gx, ref, ref.abs(), 2, route["names"][1][0], what + " gx")
-    check_sum(gb, ref.sum((0, 2, 3)), ref.abs().sum((0, 2, 3)), rowwise_c(n, c, hw, 2, False, v, sms),
+    check_sum(gb, ref.sum((0, 2, 3)), ref.abs().sum((0, 2, 3)), rowwise_c(n, c, hw, 2, False, dt, sms),
               route["names"][1][0], what + " grad_bias")
     noise = torch.randn(n, 1, shape[2], shape[3], generator=g, device=DEV)
     nw = torch.tensor([0.7], device=DEV)
@@ -652,12 +565,12 @@ def test_rowwise_nhwc(case):
     pre = x.double() * rs.double()[:, :, None, None]
     a = pre.abs() + b.double().abs()[:, None, None] + (0.7 * noise.double()).abs()
     pre = pre + b.double()[:, None, None] + 0.7 * noise.double()
-    check_stored(o, lrelu64(pre, 0.2, SQRT2), a * slope_gain(0.2, SQRT2), 5, route["noise_name"], what + " noise_bias_act")
+    check_stored(o, lrelu64(pre, A32, G32), a * slope_gain(0.2, SQRT2), 5, route["noise_name"], what + " noise_bias_act")
 
 
 def to_rgb_run(case, g):
     """Raw to-RGB forward / backward on an NHWC activation held as (N, HW, C)."""
-    L = _lib()
+    L = library()
     lib = L.load()
     n, c, hw, b, sk, want_gx, want_gwm = case
     x = torch.randn(n, hw, c, generator=g, device=DEV)
@@ -684,9 +597,9 @@ def test_to_rgb_nhwc(case):
     Backward: gx = sum_o wm*g (3 roundings, k = 3); gwm = sum_p g*x: a thread's pixels, the CTA's pixel lanes, the finish
     kernel over the K CTAs of a sample."""
     n, c, hw, b, sk, want_gx, want_gwm = case
-    sms = _lib().sm_count()
+    sms = library().sm_count()
     route = to_rgb_route(n, c, hw, sms)
-    x, wm, bias, skip, out, gy, gx, gwm = to_rgb_run(case, _gen(c + hw))
+    x, wm, bias, skip, out, gy, gx, gwm = to_rgb_run(case, seeded(c + hw))
     x64, w64, g64 = x.double(), wm.double(), gy.double()
     ref = torch.einsum("noc,npc->nop", w64, x64)
     a = torch.einsum("noc,npc->nop", w64.abs(), x64.abs())
@@ -702,7 +615,7 @@ def test_to_rgb_nhwc(case):
     if want_gwm:
         r = torch.einsum("nop,npc->noc", g64, x64)
         ra = torch.einsum("nop,npc->noc", g64.abs(), x64.abs())
-        cc = _ceil(route["bchunk"], route["lanes"]) + route["lanes"] + finish_depth(route["kb"])
+        cc = ceil_div(route["bchunk"], route["lanes"]) + route["lanes"] + finish_depth(route["kb"])
         check_sum(gwm, r, ra, cc, "to_rgb_nhwc_bwd_kernel", what + " gwm (lanes %d, K %d)" % (route["lanes"], route["kb"]))
 
 
@@ -720,7 +633,7 @@ def _poison_allocator():
 def test_empty_planes_give_zero_sums_nchw(dt):
     """A sum over an empty plane is 0: row_dot of gg_channel_scale with HW = 0, grad_bias of gg_bias_act_backward with
     N*HW = 0, and the gradient of channel_scale(x, s) w.r.t. s for an (N, C, 0, W) input."""
-    L = _lib()
+    L = library()
     lib = L.load()
     for rows, hw in ((6, 0), (1, 0)):
         dot = torch.full((rows,), float("nan"), device=DEV)
@@ -745,7 +658,7 @@ def test_empty_planes_give_zero_sums_nchw(dt):
 @pytest.mark.parametrize("dt", [F32, BF16])
 def test_empty_planes_give_zero_sums_nhwc(dt):
     """The channels-last row_dot (per sample and channel), grad_bias and the to-RGB gwm over zero pixels are 0."""
-    L = _lib()
+    L = library()
     lib = L.load()
     c = 4 * VEC[dt]
     dot = torch.full((2, c), float("nan"), device=DEV)
@@ -776,7 +689,7 @@ def test_faces_take_misaligned_constants_and_activations(dt):
     from gangealing_b200.op.feature_distance import feature_distance
     from gangealing_b200.op.modconv import _ToRGB
     from gangealing_b200.op.vgg_pool import bias_relu_pool
-    g = _gen(17)
+    g = seeded(17)
     n, c, h, w = 2, 64, 6, 4
     x = cl(randn((n, c, h, w), g, dt))
     b_all = torch.randn(c + 1, generator=g, device=DEV)
@@ -787,29 +700,29 @@ def test_faces_take_misaligned_constants_and_activations(dt):
     y = nhwc.noise_bias_act(x, None, None, b, rs, 0.2, SQRT2)
     pre = x.double() * rs.double()[:, :, None, None] + b.double()[:, None, None]
     a = (x.double() * rs.double()[:, :, None, None]).abs() + b.double().abs()[:, None, None]
-    check_stored(y, lrelu64(pre, 0.2, SQRT2), a * slope_gain(0.2, SQRT2), 5, "noise_bias_act_nhwc (face)", "offset constants")
+    check_stored(y, lrelu64(pre, A32, G32), a * slope_gain(0.2, SQRT2), 5, "noise_bias_act_nhwc (face)", "offset constants")
     y = op.fused_leaky_relu(x, b)
     bq = b.to(dt).double()[:, None, None] if dt != F32 else b.double()[:, None, None]
-    check_stored(y, lrelu64(x.double() + b.double()[:, None, None], 0.2, SQRT2),
+    check_stored(y, lrelu64(x.double() + b.double()[:, None, None], A32, G32),
                  (x.double().abs() + b.double().abs()[:, None, None]) * slope_gain(0.2, SQRT2), 5,
                  "fused_leaky_relu (face)", "offset bias")
     # a channels-last activation one element off a 16-byte boundary: the flat kernel's scalar route forward; the backward
     # gates on the (freshly allocated, aligned) output
     xl = torch.empty(1 + x.numel(), dtype=dt, device=DEV)[1:].view(n, h, w, c).permute(0, 3, 1, 2)
     xl.copy_(x)
-    assert xl.data_ptr() % 16 != 0 and _lib().is_nhwc(xl) and not nhwc.elementwise_ok(xl) and not nhwc.rowwise_ok(xl)
+    assert xl.data_ptr() % 16 != 0 and library().is_nhwc(xl) and not nhwc.elementwise_ok(xl) and not nhwc.rowwise_ok(xl)
     xl.requires_grad_(True)
     bl = b.clone().requires_grad_(True)
     y = op.fused_leaky_relu(xl, bl)
     pre = x.double() + bq
-    check_stored(y, lrelu64(pre, 0.2, SQRT2), (x.double().abs() + bq.abs()) * slope_gain(0.2, SQRT2), 3,
+    check_stored(y, lrelu64(pre, A32, G32), (x.double().abs() + bq.abs()) * slope_gain(0.2, SQRT2), 3,
                  "fused_leaky_relu (misaligned activation)", "forward")
     gy = cl(randn(y.shape, g, dt))
     gx, gb = torch.autograd.grad(y, [xl, bl], gy)
     ref = gy.double() * act_grad64(y.double())
     check_stored(gx, ref, ref.abs(), 2, "fused_leaky_relu (misaligned activation)", "gx")
     check_sum(gb.float(), ref.sum((0, 2, 3)), ref.abs().sum((0, 2, 3)),
-              rowwise_c(n, c, h * w, 2, False, VEC[dt], _lib().sm_count()), "fused_leaky_relu (misaligned activation)",
+              rowwise_c(n, c, h * w, 2, False, dt, library().sm_count()), "fused_leaky_relu (misaligned activation)",
               "grad_bias")
     if dt != F32:
         return
@@ -836,21 +749,6 @@ KERNELS = re.compile(r"(rowwise_nchw_rows_kernel|rowwise_nchw_kernel|row_finish_
                      r"rowwise_nhwc_kernel|nhwc_finish_kernel|to_rgb_nhwc_fwd_kernel|to_rgb_nhwc_bwd_kernel)(<[^>]*>)?")
 
 
-def launched(fn):
-    """Names of this family's kernels `fn` launches, in launch order, from torch.profiler's CUDA activity."""
-    from torch.profiler import ProfilerActivity, profile
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        fn()
-        torch.cuda.synchronize()
-    evs = prof.events()
-    if not any(e.device_type == torch.autograd.DeviceType.CUDA for e in evs):
-        raise RuntimeError("torch.profiler recorded no device activity (only %d runtime calls): the kernel names are "
-                           "unknown" % len(evs))
-    names = [(e.time_range.start, m.group(0)) for e in evs for m in [KERNELS.search(e.name)] if m]
-    return [nm for _, nm in sorted(names, key=lambda t: t[0])]
-
-
 @pytest.mark.gpu
 def test_routing_matches_the_restatement():
     """Every distinct route of the cases above launches the kernels (names, template arguments, order) the restatement
@@ -873,7 +771,7 @@ def test_routing_matches_the_restatement():
 
 def check_routing():
     """The body of test_routing_matches_the_restatement (raises AssertionError on a mismatch)."""
-    sms = _lib().sm_count()
+    sms = library().sm_count()
     seen, done = [], set()
 
     def expect(label, names, fn, labels=()):
@@ -882,25 +780,25 @@ def check_routing():
         if key in done:
             return
         done.add(key)
-        got = launched(fn)
+        got = launched(fn, KERNELS)
         seen.append("%-56s -> %s" % (label, got))
         assert got == names, "%s: launched %s, the restatement predicts %s" % (label, got, names)
 
     for i, case in enumerate(NCHW_CASES):
         r = nchw_rowwise_route(*case)
-        expect("nchw %s %s" % (SHORT[case[0]], case[1:]), r["names"], lambda: nchw_rowwise(case, _gen(i)), r["labels"])
+        expect("nchw %s %s" % (SHORT[case[0]], case[1:]), r["names"], lambda: nchw_rowwise(case, seeded(i)), r["labels"])
     for case in FLAT_CASES:
         dt, shape, layout, act, grad, b, xo, ro = case
         r = flat_route(dt, math.prod(shape), flat_step(shape, layout), b, grad == 1, xo, ro)
-        expect("flat %s %s %s off %d/%d" % (SHORT[dt], shape, layout, xo, ro), r["names"], lambda: flat_run(case, _gen(1)),
+        expect("flat %s %s %s off %d/%d" % (SHORT[dt], shape, layout, xo, ro), r["names"], lambda: flat_run(case, seeded(1)),
                r["labels"])
     for dt, shape, nz, nw, b, rs, xo, no in NOISE_CASES:
         r = noise_route(dt, shape[0], shape[1], shape[2] * shape[3], nz, xo, no, sms)
         expect("noise %s %s off %d/%d" % (SHORT[dt], shape, xo, no), r["names"],
-               lambda: noise_run(dt, shape, nz, nw, b, rs, xo, no, _gen(2)), r["labels"])
+               lambda: noise_run(dt, shape, nz, nw, b, rs, xo, no, seeded(2)), r["labels"])
     n, c, hw = big_scalar_shape(sms)
     r = noise_route(F32, n, c, hw, True, sms=sms)
-    expect("noise grid-stride", r["names"], lambda: noise_run(F32, (n, c, hw, 1), True, True, True, True, 0, 0, _gen(3)),
+    expect("noise grid-stride", r["names"], lambda: noise_run(F32, (n, c, hw, 1), True, True, True, True, 0, 0, seeded(3)),
            r["labels"])
     from gangealing_b200.op import nhwc
     for dt, n, c, hw in NHWC_CASES:
@@ -915,6 +813,6 @@ def check_routing():
     for case in TO_RGB_CASES:
         n, c, hw, b, sk, want_gx, want_gwm = case
         names = ["to_rgb_nhwc_fwd_kernel", "to_rgb_nhwc_bwd_kernel"] + (["nhwc_finish_kernel"] if want_gwm else [])
-        expect("to-RGB %s" % (case,), names, lambda: to_rgb_run(case, _gen(4)))
+        expect("to-RGB %s" % (case,), names, lambda: to_rgb_run(case, seeded(4)))
     for line in seen:
         print("[route] " + line)

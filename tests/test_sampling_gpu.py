@@ -4,6 +4,7 @@ import torch
 import torch.nn.functional as F
 
 from conftest import assert_close, golden_cases, load_golden
+from fp64_contract import grid_stride_batch
 from oracle import sampling as S
 
 pytestmark = pytest.mark.gpu
@@ -428,13 +429,6 @@ def test_sampler_integer_work_is_bit_exact(mode, hs, ws):
 
 
 # ------------------------------------------------------------------------------------------------ one-pass STN sampler
-def grid_stride_batch(ho, wo):
-    """A batch whose N * Ho * Wo output pixels exceed one trip of the sampler's grid-stride loops (16 CTAs of 256 threads
-    per SM: csrc/flow_compose.cuh grid_for), so that every thread makes a second trip."""
-    from gangealing_b200 import _lib
-    return _lib.sm_count() * 16 * 256 // (ho * wo) + 2
-
-
 def _kernel_grid_grad(x, grid, go, levels, mode):
     """The sampler's own backward (the kernel stn_sample_* call) on a given grid: its gradient w.r.t. the grid."""
     from gangealing_b200.stn import sampling as GS

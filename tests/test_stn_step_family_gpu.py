@@ -33,45 +33,29 @@ path when it finishes.
 import math
 import re
 import struct
-from collections import defaultdict
 
 import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
+from fp64_contract import (BF16, CODE, DEV, F32, H100_SMS, Worst, assert_routes_reached, ceil_div, f32, grid_for, launched,
+                           library, seeded)
 from oracle.rounding import U32, assert_fp32_sum
 
-DEV = "cuda"
-H100_SMS = 132
 THREADS = 256
 ADAM_CHUNK = 65536                # gangealing_b200.training.fused_optim._CHUNK
 SCALE_CHUNK = 32768               # gangealing_b200.op.scaled_weights._CHUNK
 BETAS, EPS = (0.9, 0.999), 1e-8
 DECAY = 0.5 ** (32 / 10000)
-F32, BF16 = torch.float32, torch.bfloat16
-CODE = {F32: 0, BF16: 2}
 SHORT = {F32: "f32", BF16: "bf16"}
 ESIZE = {F32: 4, BF16: 2}
 
 
-def _ceil(a, b):
-    return -(-a // b)
-
-
-def f32(v):
-    return float(np.float32(v))
-
-
 # ======================================================================================== planner restatement (no GPU)
-def grid_for(total, threads=THREADS, sms=H100_SMS):
-    """flow_compose.cuh grid_for: enough CTAs for `total` items, at most 16 per SM (grid-stride beyond that)."""
-    return min(max(_ceil(total, threads), 1), 16 * sms)
-
-
 def tv_blocks(total, sms=H100_SMS):
     """optim.cu tv_blocks: at most 4 CTAs per SM."""
-    return min(max(_ceil(total, THREADS), 1), 4 * sms)
+    return min(max(ceil_div(total, THREADS), 1), 4 * sms)
 
 
 def _trip_label(tag, total, per_trip):
@@ -119,7 +103,7 @@ def flow_bwd_route(case, sms=H100_SMS):
         warps = grid_for(entries * 32, sms=sms) * THREADS // 32
         labels.add(_trip_label("g_low entries", entries, warps))
         terms = 9 * s * s
-        labels.add("g_low lanes: %d terms, %s" % (terms, "idle lanes" if terms < 32 else "%d strides" % _ceil(terms, 32)))
+        labels.add("g_low lanes: %d terms, %s" % (terms, "idle lanes" if terms < 32 else "%d strides" % ceil_div(terms, 32)))
     if "g_base" in outs:
         if g_flow and base:
             names.append("flow_base_bwd_kernel")
@@ -127,15 +111,15 @@ def flow_bwd_route(case, sms=H100_SMS):
                                        else "several trips per thread"))
         else:
             labels.add("g_base: zeroed by the entry (%s)" % ("no g_flow" if not g_flow else "no base warp"))
-    return dict(names=names, labels=labels, lanes_chain=_ceil(9 * s * s, 32), base_trips=_ceil(per, THREADS))
+    return dict(names=names, labels=labels, lanes_chain=ceil_div(9 * s * s, 32), base_trips=ceil_div(per, THREADS))
 
 
 def tv_route(case, sms=H100_SMS):
     n, h, w, data = case
     total = n * h * w * 2
     blocks = tv_blocks(total, sms)
-    trips = _ceil(total, blocks * THREADS)
-    bwd_trips = _ceil(total, 4 * blocks * THREADS)
+    trips = ceil_div(total, blocks * THREADS)
+    bwd_trips = ceil_div(total, 4 * blocks * THREADS)
     labels = {_trip_label("tv fwd", total, blocks * THREADS), "tv data: %s" % data,
               "tv finish: %s" % ("fewer than 256 partials" if blocks < 256 else "exactly 256 partials" if blocks == 256
                                  else "two trips (more than 256 partials)"),
@@ -144,13 +128,13 @@ def tv_route(case, sms=H100_SMS):
         labels.add("tv: H = W = 2")
     if h != w:
         labels.add("tv: non-square")
-    return dict(blocks=blocks, trips=trips, finish_trips=_ceil(blocks, 256), bwd_trips=bwd_trips, labels=labels)
+    return dict(blocks=blocks, trips=trips, finish_trips=ceil_div(blocks, 256), bwd_trips=bwd_trips, labels=labels)
 
 
 def tvps_route(case):
     n, h, w, data = case
     per = h * w * 2
-    trips = _ceil(per, 512)
+    trips = ceil_div(per, 512)
     lab = "tv_per_sample: %s" % ("fewer elements than threads" if per < 512 else "elements = threads" if per == 512
                                  else "several trips per thread")
     return dict(trips=trips, labels={lab, "tv data: %s" % data})
@@ -161,7 +145,7 @@ OPERANDS = ("p", "g", "m", "v", "ema")
 
 def cta_map(numels, chunk):
     """fused_optim / scaled_weights: CTA -> (tensor, chunk) in table order."""
-    return [(ti, c) for ti, nm in enumerate(numels) for c in range(_ceil(nm, chunk))]
+    return [(ti, c) for ti, nm in enumerate(numels) for c in range(ceil_div(nm, chunk))]
 
 
 def adam_route(case):
@@ -320,11 +304,7 @@ def test_cases_reach_every_route():
     from gangealing_b200.training import fused_optim
     assert fused_optim._CHUNK == ADAM_CHUNK and scaled_weights._CHUNK == SCALE_CHUNK
     reached = all_labels()
-    missing = [lab for lab in REQUIRED if lab not in reached]
-    print("[coverage] %d of %d routes reached" % (len(REQUIRED) - len(missing), len(REQUIRED)))
-    for lab in REQUIRED:
-        print("[coverage]   %s %s" % ("ok     " if lab in reached else "MISSING", lab))
-    assert not missing, "routes no case reaches: %s" % missing
+    assert_routes_reached(REQUIRED, reached)
 
 
 def test_restated_tv_blocks_match_the_workspace_query():
@@ -339,31 +319,14 @@ def test_restated_tv_blocks_match_the_workspace_query():
 
 
 # ======================================================================================================== GPU checks
-WORST = defaultdict(float)
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _report_worst():
-    yield
-    if WORST:
-        print("\n[contract] worst observed k (stored values) / c (sums) per path:")
-        for path in sorted(WORST):
-            print("[contract]   %-48s %.2f" % (path, WORST[path]))
+WORST = Worst("k (stored values) / c (sums) per path", "%-48s %.2f")
+_report_worst = WORST.fixture()
 
 
 def check(y, ref, a, c, path, what, extra=None):
     obs = assert_fp32_sum(y, ref, a, c, "%s: %s" % (path, what), extra64=extra)
-    WORST[path] = max(WORST[path], obs)
+    WORST.note(path, obs)
     print("[contract] %s: %s: obs=%.2f (bound %g)" % (path, what, obs, c))
-
-
-def _lib():
-    from gangealing_b200 import _lib as lib
-    return lib
-
-
-def _gen(seed):
-    return torch.Generator(device=DEV).manual_seed(seed)
 
 
 def nan_like(shape):
@@ -372,7 +335,7 @@ def nan_like(shape):
 
 # ------------------------------------------------------------------------------------------------ flow composition
 def flow_inputs(n, lh, lw, s, logits, seed):
-    g = _gen(seed)
+    g = seeded(seed)
     low = torch.randn(n, lh, lw, 2, generator=g, device=DEV) * 0.3
     if logits == "narrow":
         mask = torch.randn(n, 9 * s * s, lh, lw, generator=g, device=DEV) * 0.5
@@ -462,7 +425,7 @@ def test_flow_compose_forward(case):
     delta = nan_like((n, lh * s, lw * s, 2))
     flow = nan_like((n, lh * s, lw * s, 2)) if want_flow else None
     alpha_n = None if alpha_a is None else alpha_a.expand(n).contiguous()
-    lib = _lib()
+    lib = library()
     rc = lib.load().gg_flow_compose_forward(delta.data_ptr(), lib.ptr(flow), low.data_ptr(), mask.data_ptr(),
                                             lib.ptr(ident if want_flow else None), lib.ptr(base_a), lib.ptr(alpha_n),
                                             n, lh, lw, s, lib.stream())
@@ -542,13 +505,13 @@ def flow_bwd_run(case, seed):
     n, lh, lw, s, outs, up, with_base, logits = case
     low, mask, ident, base, alpha = flow_inputs(n, lh, lw, s, logits, seed)
     base = base if with_base else None
-    g = _gen(seed + 1)
+    g = seeded(seed + 1)
     g_delta = torch.randn(n, lh * s, lw * s, 2, generator=g, device=DEV) if up in ("delta", "both") else None
     g_flow = torch.randn(n, lh * s, lw * s, 2, generator=g, device=DEV) if up in ("flow", "both") else None
     o = dict(g_mask=nan_like(mask.shape) if "g_mask" in outs else None,
              g_low=nan_like(low.shape) if "g_low" in outs else None,
              g_base=nan_like((n, 2, 3)) if "g_base" in outs else None)
-    lib = _lib()
+    lib = library()
     rc = lib.load().gg_flow_compose_backward(lib.ptr(o["g_mask"]), lib.ptr(o["g_low"]), lib.ptr(o["g_base"]), lib.ptr(g_delta),
                                              lib.ptr(g_flow), low.data_ptr(), mask.data_ptr(), ident.data_ptr(), lib.ptr(base),
                                              alpha.data_ptr(), n, lh, lw, s, lib.stream())
@@ -609,11 +572,11 @@ def test_flow_backward_faces_match_the_entry():
     low, mask, ident, base, alpha = flow_inputs(n, lh, lw, s, "narrow", 11)
     args = [t.clone().requires_grad_(True) for t in (low, mask, base)]
     d, f = flow_compose(args[0], args[1], ident, args[2], alpha, s)
-    g = _gen(12)
+    g = seeded(12)
     gd, gf = torch.randn(d.shape, generator=g, device=DEV), torch.randn(f.shape, generator=g, device=DEV)
     got = torch.autograd.grad([d, f], args, [gd, gf])
     o = dict(g_mask=torch.empty_like(mask), g_low=torch.empty_like(low), g_base=torch.empty(n, 2, 3, device=DEV))
-    lib = _lib()
+    lib = library()
     lib.check(lib.load().gg_flow_compose_backward(o["g_mask"].data_ptr(), o["g_low"].data_ptr(), o["g_base"].data_ptr(),
                                                   gd.data_ptr(), gf.data_ptr(), low.data_ptr(), mask.data_ptr(),
                                                   ident.data_ptr(), base.data_ptr(), alpha.data_ptr(), n, lh, lw, s,
@@ -639,7 +602,7 @@ def test_flow_faces_on_offset_views_match_aligned_copies():
     from gangealing_b200.stn.sampling import stn_sample_flow
     n, lh, lw, s = 2, 4, 4, 8
     low, mask, ident, base, alpha = flow_inputs(n, lh, lw, s, "narrow", 21)
-    g = _gen(22)
+    g = seeded(22)
     gd, gf = torch.randn(n, lh * s, lw * s, 2, generator=g, device=DEV), torch.randn(n, lh * s, lw * s, 2, generator=g, device=DEV)
 
     def run(lo, mk, idn, gdd, gff):
@@ -666,7 +629,7 @@ def test_sampler_faces_on_offset_views_match_aligned_copies():
     """mipmap_warp (and its grid gradient), sample_indices, mipmap_warp_lerp and mipmap_warp_lerp_mean on grids that
     start 4 bytes off give the values of the aligned copies bitwise."""
     from gangealing_b200.stn.sampling import mipmap_warp, mipmap_warp_lerp, mipmap_warp_lerp_mean, sample_indices
-    g = _gen(31)
+    g = seeded(31)
     n, ho, wo = 2, 12, 20
     img = torch.randn(n, 3, 32, 32, generator=g, device=DEV)
     grid = (torch.rand(n, ho, wo, 2, generator=g, device=DEV) * 2 - 1) * 1.1
@@ -740,7 +703,7 @@ def test_tv_loss(case):
         if dx.numel() >= 64:
             assert all(bool((dx.abs() == v).any()) for v in (1.0, 1 + 2.0 ** -23, 1 - 2.0 ** -23))
     inv_y, inv_x = tv_invs(n, h, w)
-    lib = _lib()
+    lib = library()
     dll = lib.load()
     out = nan_like((1,))
     ws = nan_like((dll.gg_tv_loss_workspace(n, h, w) // 4,))
@@ -836,7 +799,7 @@ def _grad_values(numel, gen):
 @pytest.mark.parametrize("case", ADAM_CASES, ids=lambda cs: cs[0].replace(" ", "_"))
 def test_adam_ema_step(case):
     name, spec, chunk = case
-    gen = _gen(sum(map(ord, name)))
+    gen = seeded(sum(map(ord, name)))
     lrs = [torch.tensor(1e-3, device=DEV), torch.tensor(3e-2, device=DEV)]
     rows = []
     for numel, offs, ema, grp in spec:
@@ -852,7 +815,7 @@ def test_adam_ema_step(case):
     bt = torch.tensor([t for t, _ in cmap] or [0], dtype=torch.int32, device=DEV)
     bc = torch.tensor([c for _, c in cmap] or [0], dtype=torch.int32, device=DEV)
     state = torch.tensor([0.0, float("nan"), float("nan")], device=DEV)
-    lib = _lib()
+    lib = library()
     for step, t0 in enumerate((0.0, 1.0, 998.0, 2.0 ** 24 - 2)):
         state[0] = t0
         for r in rows:
@@ -882,7 +845,7 @@ def test_fused_adam_ema_with_bucket_view_gradients():
     gradient_as_bucket_view): the kernel takes its scalar path; every step's outputs against float64 on that step's inputs,
     with two parameter groups at different learning rates."""
     from gangealing_b200.training.fused_optim import FusedAdamEMA
-    gen = _gen(41)
+    gen = seeded(41)
     shapes = [(64, 3, 3, 3), (130,), (7, 5), (ADAM_CHUNK + 3,)]
     params = [torch.randn(s, generator=gen, device=DEV).requires_grad_(True) for s in shapes]
     emas = [p.detach().clone() for p in params[:2]]
@@ -922,7 +885,7 @@ def _scale_id(cs):
 def test_scale_cast_multi(case):
     """dst == (src.float() * scale).to(dst dtype) bitwise: one correctly rounded fp32 product and one rounding to bf16."""
     name, spec = case
-    gen = _gen(sum(map(ord, name)))
+    gen = seeded(sum(map(ord, name)))
     rows, pads = [], []
     for i, (sd, dd, numel, so, do) in enumerate(spec):
         # each operand sits inside a buffer twice its size: the NaN guard bands around dst must stay NaN
@@ -933,7 +896,7 @@ def test_scale_cast_multi(case):
         scale = f32(1 / math.sqrt(9 * (i + 3)))
         rows.append((src, dst, scale))
         pads.append((dbuf, do, numel))
-    lib = _lib()
+    lib = library()
     blob = b"".join(struct.pack("<QQqfi", s.data_ptr(), d.data_ptr(), s.numel(), sc, CODE[s.dtype] | (CODE[d.dtype] << 8))
                     for s, d, sc in rows)
     table = torch.frombuffer(bytearray(blob), dtype=torch.uint8).to(DEV)
@@ -960,8 +923,8 @@ def test_flow_backward_zeroes_g_base_without_a_base_path():
     """g_base requested without g_flow, or without a base warp, is written as exact zeros by the entry itself."""
     n, lh, lw, s = 3, 2, 3, 2
     low, mask, ident, base, alpha = flow_inputs(n, lh, lw, s, "narrow", 51)
-    gd = torch.randn(n, lh * s, lw * s, 2, generator=_gen(52), device=DEV)
-    lib = _lib()
+    gd = torch.randn(n, lh * s, lw * s, 2, generator=seeded(52), device=DEV)
+    lib = library()
     for g_flow, b in ((None, base), (gd, None)):
         gb = nan_like((n, 2, 3))
         lib.check(lib.load().gg_flow_compose_backward(None, None, gb.data_ptr(), gd.data_ptr(), lib.ptr(g_flow), low.data_ptr(),
@@ -973,21 +936,6 @@ def test_flow_backward_zeroes_g_base_without_a_base_path():
 # ------------------------------------------------------------------------------------------------ launch sets
 KERNELS = re.compile(r"(flow_compose_fwd_kernel|flow_compose_bwd_kernel|flow_low_bwd_kernel|flow_base_bwd_kernel|"
                      r"tv_fwd_kernel|tv_finish_kernel|tv_bwd_kernel|adam_tick_kernel|adam_ema_kernel)")
-
-
-def launched(fn):
-    """Names of this family's kernels `fn` launches, in launch order, from torch.profiler's CUDA activity."""
-    from torch.profiler import ProfilerActivity, profile
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        fn()
-        torch.cuda.synchronize()
-    evs = prof.events()
-    if not any(e.device_type == torch.autograd.DeviceType.CUDA for e in evs):
-        raise RuntimeError("torch.profiler recorded no device activity (only %d runtime calls): the kernel names are "
-                           "unknown" % len(evs))
-    names = [(e.time_range.start, m.group(0)) for e in evs for m in [KERNELS.search(e.name)] if m]
-    return [nm for _, nm in sorted(names, key=lambda t: t[0])]
 
 
 @pytest.mark.gpu
@@ -1014,7 +962,7 @@ def check_launch_sets():
     seen = []
 
     def expect(label, names, fn):
-        got = launched(fn)
+        got = launched(fn, KERNELS)
         seen.append("%-56s -> %s" % (label, got))
         assert got == names, "%s: launched %s, the restatement predicts %s" % (label, got, names)
     done = set()
@@ -1026,7 +974,7 @@ def check_launch_sets():
         done.add(key)
         expect("flow bwd %s from %s%s" % ("+".join(cs[4]), cs[5], "" if cs[6] else " (no base)"), r["names"],
                lambda: flow_bwd_run(cs, 3))
-    lib = _lib()
+    lib = library()
     dll = lib.load()
     f = tv_flow(2, 16, 16, "random", 1)
     out = torch.empty(1, device=DEV)

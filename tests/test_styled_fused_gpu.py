@@ -4,6 +4,7 @@ import pytest
 import torch
 
 from conftest import assert_close
+from fp64_contract import BF16, blur_plan, library, lrelu64, rowwise_c, slope_gain
 from oracle import opset
 from oracle import stylegan2_ops as so
 
@@ -94,8 +95,7 @@ def _bf16_tail_contract(t, blur, xs, rgb, gg, slope=0.2, gain=2 ** 0.5):
     element it enters), and the blur layers hand g_t = lrelu'(out)*gain*g_xs*s_next from one launch to the next as a bf16
     tensor (DESIGN.md, deviations): g_raw and d_demod are allowed B^T(1/2 ulp(g_t)) on top of the fp32 bound."""
     from oracle.rounding import U32, ulp
-    from test_bf16_storage_gpu import (blur_geometry, blur_k, check_once, check_sum, fir64, lrelu64, rowwise_c,
-                                       slope_gain)
+    from test_bf16_storage_gpu import blur_k, check_once, check_sum, fir64
     d = {nm: (v.double().to(DEV) if isinstance(v, torch.Tensor) else v) for nm, v in t.items()}
     raw = t["raw"].to(torch.bfloat16).double().to(DEV)
     n, c = raw.shape[:2]
@@ -128,16 +128,16 @@ def _bf16_tail_contract(t, blur, xs, rgb, gg, slope=0.2, gain=2 ** 0.5):
         goa = goa + torch.einsum("noc,nohw->nchw", d["wm"].abs(), d["g_rgb"].abs())
     sl = torch.where(pre > 0, 1.0, slope) * gain                   # _dekink keeps every pre-activation off the kink
     gt, gta = go * sl, goa * sl.abs()
-    c_tail = rowwise_c(n, c, oh * ow, 0, True)
+    c_tail = rowwise_c(n, c, oh * ow, 0, True, BF16, library().sm_count())
     if blur:
         kf, gp = torch.flip(k, [0, 1]), (2, 2, 2, 2)
         h_t = 0.5 * ulp(gt, torch.bfloat16) + 4 * U32 * gta         # g_t: g*s, *slope, *gain, the bf16 store
         tr, tra, trh = fir64(gt, kf, gp), fir64(gta, kf.abs(), gp), fir64(h_t, kf.abs(), gp)
         check_once(gg["raw"], tr * dm, tra * dm.abs(), blur_k(k) + 1, "fused_tail g_raw (blur)", extra=trh * dm.abs())
         if "demod" in gg:
-            seg_rows, kc = blur_geometry(n, c, raw.shape[2], raw.shape[3])
+            p = blur_plan(BF16, n, c, oh, ow, 4, 4, gp, library().sm_count())
             check_sum(gg["demod"], (tr * raw).sum((2, 3)), (tra * raw.abs()).sum((2, 3)),
-                      blur_k(k) + 1 + seg_rows + 32 + kc // 32 + 35, "fused_tail d_demod (blur)", extra=(trh * raw.abs()).sum((2, 3)))
+                      blur_k(k) + 1 + p["seg_rows"] + 32 + p["xblocks"] * p["segs"] // 32 + 35, "fused_tail d_demod (blur)", extra=(trh * raw.abs()).sum((2, 3)))
     else:
         check_once(gg["raw"], gt * dm, gta * dm.abs(), 7, "fused_tail g_raw")
         if "demod" in gg:
@@ -247,7 +247,7 @@ def test_channels_last_family_in_both_storage_types(dtype):
     bf16: the storage contract against float64 (tests/test_bf16_storage_gpu.py) -- k / c stated at each check."""
     from gangealing_b200 import op
     from gangealing_b200.op.modconv import channel_scale
-    from test_bf16_storage_gpu import check_once, check_sum, fir64, rowwise_c
+    from test_bf16_storage_gpu import check_once, check_sum, fir64
     g = torch.Generator().manual_seed(7)
     lo = dtype == torch.bfloat16
     x = torch.randn(2, 128, 33, 29, generator=g)
@@ -278,7 +278,8 @@ def test_channels_last_family_in_both_storage_types(dtype):
         check_once(yg, pre * sl, (x64.abs() + b.double().to(DEV).abs()[:, None, None]) * 2 ** 0.5, 5, "fused_leaky_relu")
         sl = torch.where(yg.double() > 0, 1.0, 0.2) * 2 ** 0.5   # the backward's slope: the sign of the stored output
         check_once(gx, go64 * sl, (go64 * sl).abs(), 2, "flr grad x")
-        check_sum(gb, (go64 * sl).sum((0, 2, 3)), (go64 * sl).abs().sum((0, 2, 3)), rowwise_c(n, c, hw, 2, False), "flr grad bias")
+        check_sum(gb, (go64 * sl).sum((0, 2, 3)), (go64 * sl).abs().sum((0, 2, 3)),
+                  rowwise_c(n, c, hw, 2, False, BF16, library().sm_count()), "flr grad bias")
     else:
         assert_close(yg, yo, rtol=1e-6, what="fused_leaky_relu")
         assert_close(gx, gxo, rtol=1e-6, what="flr grad x")
@@ -293,8 +294,8 @@ def test_channels_last_family_in_both_storage_types(dtype):
         s64 = s.double().to(DEV)[:, :, None, None]
         check_once(yg, x64 * s64, (x64 * s64).abs(), 1, "channel_scale")
         check_once(gx, go64 * s64, (go64 * s64).abs(), 1, "channel_scale grad x")
-        check_sum(gs, (go64 * x64).sum((2, 3)), (go64 * x64).abs().sum((2, 3)), rowwise_c(n, c, hw, 0, True),
-                  "channel_scale grad s")
+        check_sum(gs, (go64 * x64).sum((2, 3)), (go64 * x64).abs().sum((2, 3)),
+                  rowwise_c(n, c, hw, 0, True, BF16, library().sm_count()), "channel_scale grad s")
     else:
         assert_close(yg, yo, rtol=1e-6, what="channel_scale")
         assert_close(gx, gxo, rtol=1e-6, what="channel_scale grad x")

@@ -25,35 +25,17 @@ Every check prints its worst observed k / c (`[contract] ...` lines with `pytest
 route when it finishes.
 """
 import re
-from collections import defaultdict
 
-import numpy as np
 import pytest
 import torch
 
-from oracle.rounding import U32, assert_fp32_sum, assert_rounded_once
-from test_bf16_storage_gpu import rowwise_c, rowwise_geometry
+from fp64_contract import (BF16, CODE, DEV, F32, H100_SMS, SHORT, SQRT2, TNAME, VEC, Worst, assert_routes_reached,
+                           ceil_div, f32, launched, library, nan_at, rowwise_c, rowwise_geometry, saved_output, seeded)
+from oracle.rounding import U32
 
-DEV = "cuda"
-SQRT2 = 2 ** 0.5
-H100_SMS = 132                    # SM count the CPU coverage check plans with (H100 SXM)
-F32, BF16 = torch.float32, torch.bfloat16
-VEC = {F32: 4, BF16: 8}           # channels per 16-byte access
 UNROLL = {F32: 4, BF16: 2}        # pixels in flight per thread in the backward's unrolled loop
-TNAME = {F32: "float", BF16: "__nv_bfloat16"}
-CODE = {F32: 0, BF16: 2}          # gangealing_b200._lib.GG_F32 / GG_BF16
-SHORT = {F32: "fp32", BF16: "bf16"}
 TRIP = 128                        # pixels one forward trip covers: 32 groups of 8 lanes x 4 pixels
 ABSENT = ("noise", "noise_weight", "bias", "demod", "rgb_bias", "skip")
-
-
-def _ceil(a, b):
-    return -(-a // b)
-
-
-def f32(v):
-    """A Python float as the fp32 value a kernel argument holds."""
-    return float(np.float32(v))
 
 
 def _b(v):
@@ -78,9 +60,9 @@ def fwd_route(dtype, n, c, hw, outputs, act=3, slope=0.2, gain=SQRT2, mask=False
     v = VEC[dtype]
     fast = fast_gate(act, slope, gain)
     name = "styled_tail_nhwc_kernel<%s, %s, %s>" % (TNAME[dtype], _b(fast), _b(mask))
-    k = max(1, min(_ceil(8 * sms, n), _ceil(hw, TRIP)))
-    chunk = _ceil(_ceil(hw, k), TRIP) * TRIP
-    kk = _ceil(hw, chunk)
+    k = max(1, min(ceil_div(8 * sms, n), ceil_div(hw, TRIP)))
+    chunk = ceil_div(ceil_div(hw, k), TRIP) * TRIP
+    kk = ceil_div(hw, chunk)
     j = c // (8 * v)
     last = hw - (kk - 1) * chunk                     # pixels of a sample's last CTA
     partial = last % TRIP != 0
@@ -128,7 +110,7 @@ def bwd_route(dtype, n, c, hw, g_xs, g_rgb, ds, dd, dwm, mask=False, layout="pac
     lanes, chunk, kk = rowwise_geometry(n, cv, hw, sms)
     lens = {chunk, hw - (kk - 1) * chunk}
     unrolled = max(lens) > (u - 1) * lanes           # pp + (U-1)*lanes_p < p1 for the first pixel lane
-    remainder = any(_ceil(m - pl, lanes) % u for m in lens for pl in range(min(lanes, m)))
+    remainder = any(ceil_div(m - pl, lanes) % u for m in lens for pl in range(min(lanes, m)))
     name = "styled_tail_bwd_nhwc_kernel<%s, %s>" % (TNAME[dtype], _b(mask))
     r = ds + dd + 3 * dwm
     if r == 0:
@@ -212,7 +194,7 @@ def bwd_geometry(dt, cv, sms=H100_SMS):
     lanes = max(256 // cv, 1)
     c = cv * VEC[dt]
     u = UNROLL[dt]
-    k5 = _ceil(8 * sms, 5)
+    k5 = ceil_div(8 * sms, 5)
     return [(1, c, 4 * lanes - 1), (5, c, 7 * u * lanes + 3), (3, c, (u - 1) * lanes), (2, c, k5 * 2 * u * lanes + 5)]
 
 
@@ -305,11 +287,7 @@ def test_cases_reach_every_route():
     reached = set()
     for r in all_routes():
         reached |= r["labels"]
-    missing = [lab for lab in REQUIRED if lab not in reached]
-    print("[coverage] %d of %d routes reached" % (len(REQUIRED) - len(missing), len(REQUIRED)))
-    for lab in REQUIRED:
-        print("[coverage]   %s %s" % ("ok     " if lab in reached else "MISSING", lab))
-    assert not missing, "routes no case reaches: %s" % missing
+    assert_routes_reached(REQUIRED, reached)
 
 
 def test_restated_geometry_matches_the_workspace_query():
@@ -342,46 +320,9 @@ def test_bad_reduce_pitch_is_refused_before_any_device_work():
 
 
 # ======================================================================================================== GPU checks
-WORST = defaultdict(float)
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _report_worst():
-    yield
-    if WORST:
-        print("\n[contract] worst observed k (stored values) / c (sums) per route:")
-        for path in sorted(WORST):
-            print("[contract]   %-64s %.2f" % (path, WORST[path]))
-
-
-def check_stored(y, ref, a, k, path, what):
-    """A stored value: fp32 within k * 2^-24 * A; bf16 within 1/2 ulp + k * 2^-24 * A."""
-    if y.dtype == F32:
-        obs = assert_fp32_sum(y, ref, a, k, "%s: %s" % (path, what))
-    else:
-        _, obs = assert_rounded_once(y, ref, a, k, "%s: %s" % (path, what))
-    WORST[path + " (k)"] = max(WORST[path + " (k)"], obs)
-    print("[contract] %s: %s: k_obs=%.2f (k=%d)" % (path, what, obs, k))
-
-
-def check_sum(y, ref, a, c, path, what):
-    obs = assert_fp32_sum(y, ref, a, c, "%s: %s" % (path, what))
-    WORST[path + " (c)"] = max(WORST[path + " (c)"], obs)
-    print("[contract] %s: %s: c_obs=%.2f (c=%d)" % (path, what, obs, c))
-
-
-def _gen(seed):
-    return torch.Generator(device=DEV).manual_seed(seed)
-
-
-def _lib():
-    from gangealing_b200 import _lib as lib
-    return lib
-
-
-def nan_at(shape, dtype):
-    """An output buffer filled with NaN: an element no launch writes stays NaN."""
-    return torch.full(shape, float("nan"), dtype=dtype, device=DEV)
+WORST = Worst("k (stored values) / c (sums) per route")
+_report_worst = WORST.fixture()
+check_stored, check_sum = WORST.check_stored, WORST.check_sum
 
 
 def unpack_mask(words, c):
@@ -406,7 +347,7 @@ def fwd_k(case, fast):
 
 def fwd_inputs(case, seed):
     dt, n, c, hw, outs, ab, act, slope, gain, mask = case
-    g = _gen(seed)
+    g = seeded(seed)
     t = dict(raw=torch.randn(n, hw, c, generator=g, device=DEV).to(dt),
              noise=None if "noise" in ab else torch.randn(n, hw, generator=g, device=DEV),
              nw=None if "noise_weight" in ab else torch.tensor([0.3], device=DEV),   # kept without noise: ignored then
@@ -452,7 +393,7 @@ def _dekink(t, dt):
 def fwd_run(case, t):
     """One FWD_CASES entry through the C ABI into NaN-filled outputs -> (out or mask, xs, rgb)."""
     dt, n, c, hw, outs, ab, act, slope, gain, mask = case
-    L = _lib()
+    L = library()
     lib = L.load()
     out = None
     if "out" in outs:
@@ -479,7 +420,7 @@ def test_styled_tail_forward(case):
     channel vectors, 3 butterfly steps, + rgb_bias, + skip, on o's fwd_k roundings -> c = C/8 + 5 + fwd_k.  The sign mask:
     each bit equals the sign of the float64 o wherever |o| exceeds o's rounding bound."""
     dt, n, c, hw, outs, ab, act, slope, gain, mask = case
-    sms = _lib().sm_count()
+    sms = library().sm_count()
     route = fwd_route_of(case, sms)
     path = route["name"]
     t = fwd_inputs(case, c + hw + 7 * n + int(100 * slope) + 13 * act)
@@ -523,12 +464,6 @@ def bwd_k(gx, gr):
     return (1 if gx else 0) + (3 if gr else 0) + 2
 
 
-def saved_output(shape, g, dtype):
-    """A forward output to gate on: mixed signs and ~5 % exact zeros (o > 0 is strict: lrelu'(0) takes the slope)."""
-    t = torch.randn(shape, generator=g, device=DEV)
-    return torch.where(torch.rand(shape, generator=g, device=DEV) < 0.05, torch.zeros_like(t), t).to(dtype)
-
-
 def sum_outputs(n, c, ds, dd, dwm, layout):
     """NaN-filled destinations: one (N, r, C) block (packed) or separate dense tensors carved from one buffer with gaps
     between them, so that they can never be mistaken for a packed block -> (d_s, d_d, d_w, reduce_pitch)."""
@@ -560,9 +495,9 @@ def sum_outputs(n, c, ds, dd, dwm, layout):
 
 def bwd_run(case, seed):
     dt, n, c, hw, gx, gr, ds, dd, dwm, mask, layout, slope, gain, has_demod = case
-    L = _lib()
+    L = library()
     lib = L.load()
-    g = _gen(seed)
+    g = seeded(seed)
     t = dict(g_xs=torch.randn(n, hw, c, generator=g, device=DEV).to(dt) if gx else None,
              g_rgb=torch.randn(n, 3, hw, generator=g, device=DEV) if gr else None,
              s_next=torch.randn(n, c, generator=g, device=DEV) + 1.0 if gx else None,
@@ -608,7 +543,7 @@ def test_styled_tail_backward(case):
     sum g_t*raw (that c + bwd_k, the roundings of g_t).  lrelu' comes from the saved activation (general route: ~5 % exact
     zeros take the slope) or from the sign mask (MASK route: random bits)."""
     dt, n, c, hw, gx, gr, ds, dd, dwm, mask, layout, slope, gain, has_demod = case
-    sms = _lib().sm_count()
+    sms = library().sm_count()
     route = bwd_route_of(case, sms)
     path = route["name"]
     t, g_raw, d_s, d_d, d_w = bwd_run(case, c + hw + 3 * n + 5 * ds + 7 * dd + 11 * dwm)
@@ -633,7 +568,7 @@ def test_styled_tail_backward(case):
     if mask:
         return
     # a thread's fma chain over its pixels, the CTA's pixel lanes in order, nhwc_finish_kernel over a sample's K CTAs
-    cc = rowwise_c(n, c, hw, 0, True, VEC[dt], sms)
+    cc = rowwise_c(n, c, hw, 0, True, dt, sms)
     o64 = t["out"].double()
     fin = route["finish"]
     if ds:
@@ -663,7 +598,7 @@ def test_empty_planes_give_zero_sums(dt):
     """d_s_next, d_demod and d_wm over zero pixels (HW = 0, N*C > 0) are 0: through the Python face, and through the C ABI
     into a packed block and into separate outputs (reduce_pitch C and 0).  N = 0 writes nothing."""
     from gangealing_b200.op import nhwc
-    L = _lib()
+    L = library()
     lib = L.load()
     n, c = 2, 8 * VEC[dt]
     empty = torch.empty(n, c, 0, 5, dtype=dt, device=DEV).contiguous(memory_format=torch.channels_last)
@@ -696,7 +631,7 @@ def test_empty_planes_give_zero_sums(dt):
 def test_bad_reduce_pitch_leaves_every_output_untouched(dt):
     """A reduce_pitch other than 0, C or r*C returns -1 before the main kernel is launched: g_raw and the sums keep their
     NaN fill."""
-    L = _lib()
+    L = library()
     lib = L.load()
     n, c, hw = 2, 8 * VEC[dt], 300
     case = (dt, n, c, hw, True, True, 1, 1, 1, False, "dense", 0.2, SQRT2, True)
@@ -732,9 +667,9 @@ def test_faces_refuse_activations_the_kernels_cannot_read(dt):
     """styled_tail and styled_tail_backward raise before any launch when raw, out_saved or g_xs is not a 16-byte-aligned
     channels-last tensor of the activation's shape and dtype (or g_rgb not dense fp32 (N, 3, H, W))."""
     from gangealing_b200.op import nhwc
-    L = _lib()
+    L = library()
     n, c, h, w = 2, 8 * VEC[dt], 5, 6
-    g = _gen(5)
+    g = seeded(5)
     cl = torch.channels_last
     raw = torch.randn(n, c, h, w, generator=g, device=DEV).to(dt).contiguous(memory_format=cl)
     out = raw.clone(memory_format=cl)
@@ -770,21 +705,6 @@ def test_faces_refuse_activations_the_kernels_cannot_read(dt):
 KERNELS = re.compile(r"(styled_tail_nhwc_kernel|styled_tail_bwd_nhwc_kernel|nhwc_finish_kernel)(<[^>]*>)?")
 
 
-def launched(fn):
-    """Names of this family's kernels `fn` launches, in launch order, from torch.profiler's CUDA activity."""
-    from torch.profiler import ProfilerActivity, profile
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        fn()
-        torch.cuda.synchronize()
-    evs = prof.events()
-    if not any(e.device_type == torch.autograd.DeviceType.CUDA for e in evs):
-        raise RuntimeError("torch.profiler recorded no device activity (only %d runtime calls): the kernel names are "
-                           "unknown" % len(evs))
-    names = [(e.time_range.start, m.group(0)) for e in evs for m in [KERNELS.search(e.name)] if m]
-    return [nm for _, nm in sorted(names, key=lambda t: t[0])]
-
-
 @pytest.mark.gpu
 def test_routing_matches_the_restatement():
     """Every distinct route of the cases above launches the kernels (names, template arguments, number of finish
@@ -806,14 +726,14 @@ def test_routing_matches_the_restatement():
 
 def check_routing():
     """The body of test_routing_matches_the_restatement (raises AssertionError on a mismatch)."""
-    sms = _lib().sm_count()
+    sms = library().sm_count()
     seen, done = [], set()
 
     def expect(label, key, names, fn):
         if key in done:
             return
         done.add(key)
-        got = launched(fn)
+        got = launched(fn, KERNELS)
         seen.append("%-72s -> %s" % (label, got))
         assert got == names, "%s: launched %s, the restatement predicts %s" % (label, got, names)
 

@@ -4,8 +4,8 @@ import pytest
 import torch
 
 from conftest import assert_close, golden_cases, load_golden
+from demod_reference import DEMOD_CASES, DEMOD_RTOL, demod_inputs, demod_ref, max_rel_err
 from oracle import stylegan2_ops as so
-from test_demod_precision import DEMOD_CASES, DEMOD_RTOL, demod_inputs, demod_ref, max_rel_err
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"

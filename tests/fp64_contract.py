@@ -126,18 +126,23 @@ class Worst:
         print("[contract] %s: %s: c_obs=%.2f (c=%d)" % (path, what, obs, c))
 
 
-def launched(fn, kernels):
+def launched(fn, kernels, sessions=3):
     """Names matching the compiled regex `kernels` of the kernels `fn` launches, in launch order, from torch.profiler's
-    CUDA activity."""
+    CUDA activity.  torch.profiler at times records a session's runtime calls without any device activity at all; such a
+    session says nothing about the kernels, so it is repeated, up to `sessions` in all (`fn` launches the same kernels
+    each time it runs).  A session with device activity is never repeated: its names are the answer."""
     from torch.profiler import ProfilerActivity, profile
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        fn()
+    for _ in range(sessions):
         torch.cuda.synchronize()
-    evs = prof.events()
-    if not any(e.device_type == torch.autograd.DeviceType.CUDA for e in evs):
-        raise RuntimeError("torch.profiler recorded no device activity (only %d runtime calls): the kernel names are "
-                           "unknown" % len(evs))
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            fn()
+            torch.cuda.synchronize()
+        evs = prof.events()
+        if any(e.device_type == torch.autograd.DeviceType.CUDA for e in evs):
+            break
+    else:
+        raise RuntimeError("torch.profiler recorded no device activity in %d sessions (only %d runtime calls in the last): "
+                           "the kernel names are unknown" % (sessions, len(evs)))
     names = [(e.time_range.start, m.group(0)) for e in evs for m in [kernels.search(e.name)] if m]
     return [nm for _, nm in sorted(names, key=lambda t: t[0])]
 

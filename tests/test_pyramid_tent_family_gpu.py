@@ -25,8 +25,8 @@ Single-level reads use separable grids whose entries are multiples of 2^-12, so 
 fp32.  The level of detail measures neighbour distances with a (size - 1) / 2 scale: where size - 1 is a power of two
 on an axis, the grid step places neighbours exactly 2^L px apart and the level of detail alone yields level L.  For
 other sizes no dyadic step can do that, so the same grid keeps the distance just under 2^L and min_level = L pins the
-level; either way w = 0 and l0 = l1 = L, asserted through the returned levels.  How the level of detail is chosen stays
-with test_sampling_gpu.py.
+level; either way w = 0 and l0 = l1 = L, asserted through the returned levels.  How the level of detail is chosen, and
+the sampler between levels, is checked against float64 by test_warp_family_gpu.py.
 
 Every check prints its worst observed c (`[contract] ...` lines with `pytest -s`), and the module prints the worst per
 path when it finishes.

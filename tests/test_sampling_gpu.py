@@ -6,6 +6,7 @@ import torch.nn.functional as F
 from conftest import assert_close, golden_cases, load_golden
 from fp64_contract import grid_stride_batch
 from oracle import sampling as S
+from warp_reference import _edge_grid, coordinate_decided, level_atol, level_decided, neighbour_sq, undecided_pixels
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -22,96 +23,8 @@ def _stn():
 LOW_PRECISION_TOL = {torch.float32: 3e-4, torch.float16: 1e-3, torch.bfloat16: 8e-3}
 
 
-def level_atol(size):
-    """levels vs the float64 oracle: the level of detail is log2 of a difference of fp32 coordinates of up to ~size px,
-    which cancellation leaves with ~ulp(coordinate) / distance relative error: measured 3e-5 (128 px source) and 1.6e-4
-    (512 px) in log2 units at 1-2 px distances."""
-    return 1e-4 * max(1.0, size / 200.0)
-
-
-# ------------------------------------------------------------------------------------------------ "decided" pixels
-# The sampler makes discrete choices: the bilinear corner floor(c), the mip levels floor / ceil(level), the arg-max
-# neighbour of the level of detail and the clamps of both.  Where the oracle's value sits within rounding noise of such a
-# boundary, the last ulp of the fp32 evaluation order decides the choice (on the GPU as in ATen's own CUDA kernel), and the
-# grid gradient jumps there.  Those pixels are exempt from the grid-gradient comparisons; the exempt set must stay tiny.
-# The level thresholds are those of the fp32 level of detail (level_atol): level_atol of a level, half of it relative
-# between the two largest neighbour distances.
-def coordinate_decided(c, size, mode, exact_integers=False):
-    """floor(c) is decided: c is not within 1e-4 px of an integer -- or pinned to a border pixel by the clamp of the border /
-    reflection modes (an exact constant on both sides).  `exact_integers`: c is the float64 image of fp32 arithmetic that is
-    exact on both sides (dyadic grids; float64 of fp32 inputs, where an exact integer is an exact integer in fp32 too)."""
-    off = (c - c.round()).abs()
-    ok = off > 1e-4
-    if exact_integers:
-        ok |= off == 0
-    if mode != "zeros":
-        ok |= (c == 0) | (c == size - 1)
-    return ok
-
-
-def level_decided(lv):
-    """floor / ceil of a level of detail are decided: not within 1e-5 of an integer -- or exactly 0, the clamp of a
-    distance <= 1 px (an exact constant on both sides)."""
-    return ((lv - lv.round()).abs() > 1e-5) | (lv == 0)
-
-
-def neighbour_sq(grid, hs, ws):
-    """(4, N, Ho, Wo) squared distances, in level-of-detail coordinates, to the left / right / up / down neighbour
-    (replicate-clamped at the image border), unclamped -- the oracle's max_coord_distance before its clamp(min=1)."""
-    c = S.lod_coordinates(grid, hs, ws)
-    p = F.pad(c.permute(0, 3, 1, 2), (1, 1, 1, 1), mode="replicate").permute(0, 2, 3, 1)
-    neigh = [p[:, 1:-1, :-2], p[:, 1:-1, 2:], p[:, :-2, 1:-1], p[:, 2:, 1:-1]]
-    return torch.stack([((o - c) ** 2).sum(dim=3) for o in neigh])
-
-
-def _mark_targets(bad, nb_idx, sel):
-    """bad |= the neighbours nb_idx (0 left, 1 right, 2 up, 3 down; replicate-clamped) of the pixels `sel`."""
-    n, ho, wo = bad.shape
-    ni, yi, xi = torch.meshgrid(torch.arange(n), torch.arange(ho), torch.arange(wo), indexing="ij")
-    ty = (yi + torch.tensor([0, 0, -1, 1])[nb_idx]).clamp(0, ho - 1)
-    tx = (xi + torch.tensor([-1, 1, 0, 0])[nb_idx]).clamp(0, wo - 1)
-    bad[ni[sel], ty[sel], tx[sel]] = True
-
-
-def undecided_pixels(grid, hs, ws, mode, max_level=None, min_level=0.0, grid_gradient=True):
-    """(N, Ho, Wo) bool, from the float64 grid: a bilinear coordinate within 1e-4 px of an integer, or (mip sampling,
-    `max_level` not None) the level within level_atol of an integer or of a clamp, or the top two neighbour distances within
-    half of that relative, or (border / reflection) the coordinate within 1e-4 px of the clip.  Exactly-on values are
-    decided: the float64 images of fp32 inputs are exact, and so are their ties.
-    `grid_gradient`: a pixel also receives the level-of-detail term of every neighbour that targets it, so an undecided
-    level or arg-max also marks every neighbour that may be the arg-max (a corner index only moves the
-    pixel's own terms: the level-of-detail term is continuous in it)."""
-    g = grid.double()
-    bad = torch.zeros(g.shape[:3], dtype=torch.bool)
-    for k, size in ((0, ws), (1, hs)):
-        bad |= ~coordinate_decided(S.source_index(g[..., k], size, mode), size, mode, True)
-        if mode != "zeros":     # the clip itself: a coordinate at the border is clamped (gradient 0) on one side only
-            raw = ((g[..., k] + 1.0) * size - 1.0) / 2.0
-            raw = S._reflect(raw, -1, 2 * size - 1) if mode == "reflection" else raw
-            for edge in (0.0, size - 1.0):
-                bad |= ((raw - edge).abs() <= 1e-4) & (raw != edge)
-    if max_level is None:
-        return bad
-    sq = neighbour_sq(g, hs, ws)
-    raw = 0.5 * torch.log2(sq.max(dim=0).values)          # unclamped level; -inf where every neighbour coincides
-    off = (raw - raw.round()).abs()
-    tol = level_atol(max(hs, ws))
-    level_bad = (off > 0) & (off <= tol) & (raw >= -tol) & (raw <= max_level + tol)
-    for clamp in (max_level, min_level):
-        level_bad |= (raw != clamp) & ((raw - clamp).abs() <= tol)
-    top = sq.clamp(min=1.0).sqrt().topk(2, dim=0)
-    gap = top.values[0] - top.values[1]
-    tie_bad = (gap > 0) & (gap <= 0.5 * tol * top.values[0])
-    bad |= level_bad | tie_bad
-    if grid_gradient:
-        # the kernel's arg-max may be ANY neighbour whose distance lies within the rounding band of the largest (three of them
-        # can be that close), judged by the UNCLAMPED distance: below 1 px the clamp ties them all, the rounding does not
-        band = sq >= sq.max(dim=0).values * (1.0 - tol)
-        for k in range(4):
-            _mark_targets(bad, torch.full(bad.shape, k), (level_bad | tie_bad) & band[k])
-    return bad
-
-
+# level_atol, the "decided" pixels (coordinate_decided, level_decided, undecided_pixels), neighbour_sq and the constructed
+# edge grids (_edge_grid) live in warp_reference.py, which test_warp_family_gpu.py shares.
 def warp_oracle(x, grid, go, num_levels, min_level, mode):
     """float64 autograd of the oracle on the kernel's inputs (x, grid, go as the kernel sees them) ->
     out, levels, grad_x, grad_grid, and grad_grid with the levels detached (the bilinear part alone)."""
@@ -224,49 +137,6 @@ def _check_training_shape(size, res, mode, dtype):
 
 # grid-gradient tolerances, relative to the largest entry of the whole gradient / of its level-of-detail share
 GRID_RTOL, LOD_RTOL = 1e-4, 1e-4
-
-
-def _dyadic(k):
-    return k.double() / 512.0
-
-
-def _edge_grid(case):
-    """Constructed grids (N, Ho, Wo, 2), source size and sampler settings for the edges of the grid-gradient gather."""
-    yy, xx = torch.meshgrid(torch.arange(16), torch.arange(16), indexing="ij")
-    if case == "pinch":
-        # a zoomed-out dyadic affine grid (~4 px between neighbours) with three points displaced ~20 px: every neighbour of
-        # the displaced interior point (4), edge point (3) and corner point (2) takes it as its arg-max neighbour
-        k = torch.stack([64 * xx + 9 * yy - 540, -6 * xx + 60 * yy - 480], dim=-1)
-        for y, x in ((8, 8), (0, 5), (15, 15)):
-            k[y, x] += torch.tensor([256, -205])
-        return _dyadic(k[None]).float(), 64, 8, 0.0
-    if case == "ties":
-        # dyadic affine grid (k/512): left/right and up/down distances tie EXACTLY (in fp32 too), half the pixels nudged by
-        # +-1/512 so that some ties break; "first maximum, order left, right, up, down" = torch.max(dim=0)'s first index
-        g = torch.Generator().manual_seed(5)
-        kx = 40 * xx + 13 * yy - 300
-        ky = -11 * xx + 37 * yy - 280
-        k = torch.stack([kx, ky], dim=-1) + torch.randint(-1, 2, (16, 16, 2), generator=g) * (torch.rand(16, 16, 1, generator=g) < 0.5)
-        return _dyadic(k[None]).float(), 64, 8, 0.0
-    if case.startswith("clamps"):
-        # 65 px source: level-of-detail coordinates are k/16 + 32, so steps of 16, 24, 32, 48, 64, 128 (/512) are distances
-        # of exactly 1 (sq == 1: level 0 at the clamp), 1.5, 2, 3, 4 (level 2 = min_level of "clamps_min") and 8 px
-        # (level 3 = max_level); a corner patch has unit steps only, the
-        # crossing of rows and columns 10..13 4 px steps only
-        g = torch.Generator().manual_seed(6)
-        steps = torch.tensor([16, 24, 32, 48, 64, 128])
-        sx, sy = steps[torch.randint(0, 6, (16, 16), generator=g)], steps[torch.randint(0, 6, (16, 16), generator=g)]
-        sx[:4, :4] = sy[:4, :4] = 16
-        sx[10:14, :] = 64
-        sy[:, 10:14] = 64
-        kx, ky = sx.cumsum(1), sy.cumsum(0)
-        k = torch.stack([kx - kx[8, 8], ky - ky[8, 8]], dim=-1)
-        return _dyadic(k[None]).float(), 65, 4, (2.0 if case == "clamps_min" else 0.0)
-    # "borders": source coordinates exactly on (and just inside / outside of) both borders: k = -504 / 504 is c = 0 / 63
-    # on a 64 px source, k = -512 / 512 the edges of the normalised range (reflection folds them onto the borders)
-    kx = torch.where(xx < 8, -528 + 4 * xx, 488 + 4 * (xx - 8))
-    ky = -504 + 84 * yy
-    return _dyadic(torch.stack([kx, ky], dim=-1)[None]).float(), 64, 8, 0.0
 
 
 @pytest.mark.parametrize("mode", S.PAD_MODES)

@@ -111,6 +111,49 @@ def injected_draws(initial, draws, record=None):
         torch.randint, torch.multinomial = randint, multinomial
 
 
+def kmeans_setup(device, ops):
+    """The fixture's generator, perceptual loss and latents, built with this package's modules."""
+    from gangealing_b200.stylegan2 import Generator
+    from gangealing_b200.training.perceptual import PerceptualLoss
+    G = kmeans_generator(Generator, ops=ops).to(device)
+    loss = opset.fill_convs_in_order(PerceptualLoss(ops=ops), KMEANS["vgg_seed"]).to(device)
+    if device != "cpu":
+        loss = loss.to(memory_format=torch.channels_last)
+    return G, loss, kmeans_w().to(device)
+
+
+def run_kmeans(blob, device, ops):
+    """This package's kmeans_plusplus with the draws stored in `blob` (the loaded fixture) injected -> (latents,
+    centroids, per-round distances, per-round probabilities)."""
+    from gangealing_b200.training.latent_learner import kmeans_plusplus
+    k = KMEANS
+    G, loss, w = kmeans_setup(device, ops)
+    dists, probs = [], []
+
+    def loss_fn(a, b):
+        d = loss(a, b)
+        dists.append(d.detach().reshape(-1).cpu())
+        return d
+
+    draws = blob["kmeans.draws"]
+    with injected_draws(int(draws[0]), [int(v) for v in draws[1:]]):
+        inner = torch.multinomial
+
+        def spy(p, num_samples=1, **kw):       # records each round's probabilities, then returns the stored draw
+            probs.append(p.detach().cpu())
+            return inner(p, num_samples, **kw)
+
+        torch.multinomial = spy
+        try:
+            centroids = kmeans_plusplus(k["num_heads"], k["num_latent"], FixedLatents(G, w), loss_fn, k["inject_index"],
+                                        k["batch_size"])
+        finally:
+            torch.multinomial = inner
+    per_round = -(-k["num_latent"] // k["batch_size"])
+    rounds = torch.stack([torch.cat(dists[r * per_round:(r + 1) * per_round]) for r in range(k["num_heads"] - 1)])
+    return w, centroids, rounds, torch.stack(probs)
+
+
 def gen_pca(ref_ll, out):
     for name, n, d, k, n_upd, seed in PCA_CASES:
         w = case_latents(seed, n + n_upd + ENCODE_ROWS, d)

@@ -2,20 +2,30 @@
 
 Each family module restates in Python how the library plans its launches, labels its cases with the routes they take, and
 checks every output against float64 with a bound derived from the kernel's operation order (oracle/rounding.py).  This
-module holds the pieces they have in common: the dtype tables, small input helpers, the registry of the worst observed
-k / c that a module prints when it finishes, the kernel-name probe, the coverage assertion, and the one restatement of
-each C launch planner that more than one module plans with:
+module holds the pieces they have in common:
+
+  the dtype tables and small input helpers (randn, at_offset, nan_at, cl, ...)
+  the checks: the registry of the worst observed k / c that a module prints when it finishes (Worst), the unregistered
+    checks that print each ratio (check_once, check_sum), the coverage assertion
+  the kernel-name probe (launched) and the fresh interpreter a module's launch check runs in (run_fresh)
+  the float64 references and bounds more than one module checks with: fir64 and blur_k (blurs), distance64 and
+    distance_forward_c (the perceptual feature distance)
+  the one restatement of each C launch planner that more than one module plans with:
 
   blur_plan          csrc/nhwc.cu blur_plan
   rowwise_geometry   csrc/nhwc.cu rowwise_chunk and csrc/styled.cu bwd_chunk (rowwise_c, finish_depth: their sums)
   grid_for           csrc/flow_compose.cuh grid_for (grid_stride_batch: a batch that takes two of its trips)
 """
 import math
+import os
+import subprocess
+import sys
 from collections import defaultdict
 
 import numpy as np
 import pytest
 import torch
+import torch.nn.functional as F
 
 from oracle.rounding import assert_fp32_sum, assert_rounded_once
 
@@ -57,6 +67,10 @@ def at_offset(t, off):
     return v
 
 
+def cl(t):
+    return t.contiguous(memory_format=torch.channels_last)
+
+
 def randn(shape, g, dtype=F32, off=0):
     t = torch.randn(shape, generator=g, device=DEV).to(dtype)
     return at_offset(t, off) if off else t
@@ -86,6 +100,16 @@ def slope_gain(slope, gain):
 
 
 # ======================================================================================================== the checks
+def check_once(y, ref, a, k, what, extra=None):
+    ulps, k_obs = assert_rounded_once(y, ref, a, k, what, extra)
+    print("[contract] %s: %.4f ulp, k_obs=%.2f (k=%g)" % (what, ulps, k_obs, k))
+
+
+def check_sum(y, ref, a, c, what, extra=None):
+    r = assert_fp32_sum(y, ref, a, c, what, extra)
+    print("[contract] %s: c_obs=%.2f (c=%d)" % (what, r, c))
+
+
 class Worst:
     """The worst observed k (stored values) / c (sums) per path of one test module.  The module registers the report
     that prints them when its tests finish with `_report_worst = WORST.fixture()` (a fixture has to live in the module).
@@ -147,6 +171,21 @@ def launched(fn, kernels, sessions=3):
     return [nm for _, nm in sorted(names, key=lambda t: t[0])]
 
 
+def run_fresh(module, function, timeout=900):
+    """Run `function` of the test module `module` in a fresh interpreter, print its output and fail if it fails.  The
+    launch checks that read kernel names run there: in a process that has already run other GPU tests, torch.profiler
+    can record the runtime calls (cudaLaunchKernel) without any kernel activity, so the names could not be read."""
+    here = os.path.dirname(os.path.abspath(__file__))
+    root = os.path.dirname(here)
+    env = dict(os.environ)
+    env["PYTHONPATH"] = os.pathsep.join([here, root] + ([env["PYTHONPATH"]] if env.get("PYTHONPATH") else []))
+    flags = ["-s"] if sys.flags.no_user_site else []
+    proc = subprocess.run([sys.executable] + flags + ["-c", "import %s as t; t.%s()" % (module, function)],
+                          cwd=root, env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=timeout)
+    print(proc.stdout)
+    assert proc.returncode == 0, "%s.%s failed:\n%s" % (module, function, proc.stdout[-6000:])
+
+
 def assert_routes_reached(required, reached, unreached=(), noun="routes"):
     """Print which of the `required` route labels the cases reach ([coverage] lines, with `pytest -s`) and those known
     to stay unreached, then assert that none is missing."""
@@ -157,6 +196,72 @@ def assert_routes_reached(required, reached, unreached=(), noun="routes"):
     for lab in unreached:
         print("[coverage]   unreached %s" % lab)
     assert not missing, "%s no case reaches: %s" % (noun, missing)
+
+
+# ============================================================================================ float64 references, bounds
+def fir64(x, k, pad):
+    """upfirdn2d(up = down = 1) in float64: TRUE convolution with `k` (upfirdn2d.py:185-187), pad = (x0, x1, y0, y1)."""
+    xp = F.pad(x, list(pad))
+    kh, kw = k.shape
+    oh, ow = xp.shape[2] - kh + 1, xp.shape[3] - kw + 1
+    kf = torch.flip(k.double(), [0, 1]).tolist()
+    out = torch.zeros(x.shape[0], x.shape[1], oh, ow, dtype=torch.float64, device=x.device)
+    for a in range(kh):
+        for b in range(kw):
+            out += kf[a][b] * xp[:, :, a:a + oh, b:b + ow]
+    return out
+
+
+def blur_k(kernel):
+    """fp32 roundings of one blurred value: separable = 4 horizontal + 4 vertical products/sums + the factorised column
+    taps (col / pivot); otherwise 16 fused multiply-adds."""
+    from gangealing_b200 import _lib
+    return 9 if _lib.filter_is_separable(kernel) else 16
+
+
+def distance_c_terms(c):
+    """(S, e_ia, TRIPS, L): S = roundings of a pixel's sum of squares (a lane's 4*TRIPS fmas + log2(L) butterfly steps),
+    e_ia = roundings in 1/(sqrt(S) + eps) (S/2 through the square root, sqrt, + eps, the division)."""
+    c4 = c // 4
+    L = min(32, c4)
+    trips = c4 // L
+    s = 4 * trips + int(math.log2(L))
+    return s, s / 2 + 3, trips, L
+
+
+def distance_forward_c(n, c, hw):
+    """distance value: 2*(e_ia + 2) for the squared normalised difference, a lane's fmas and its pixels (chunk / groups),
+    the warp sum (5), the CTA's 8 warps, *1/HW (2), the finish kernel's K partials."""
+    s, e_ia, trips, L = distance_c_terms(c)
+    groups = 256 // L
+    k = max(1, min(ceil_div(8 * library().sm_count(), n), ceil_div(hw, 2 * groups), 64))
+    chunk = ceil_div(hw, k)
+    return int(math.ceil(2 * (e_ia + 2) + 4 * trips + ceil_div(chunk, groups) + 5 + 8 + 2 + ceil_div(hw, chunk)))
+
+
+def distance64(a, b, w, gout, eps=1e-10):
+    """float64 feature distance of the stored maps a, b (N, C, H, W), its value on absolute values, and the gradients with
+    their absolute-value counterparts.  A pixel whose map is all zero gets gradient 0 (csrc/lpips.cu)."""
+    hw = a.shape[2] * a.shape[3]
+    wv = w.double().reshape(1, -1, 1, 1) if w is not None else torch.ones(1, a.shape[1], 1, 1, dtype=torch.float64, device=a.device)
+    ra = a.square().sum(1, keepdim=True).sqrt()
+    rb = b.square().sum(1, keepdim=True).sqrt()
+    ia, ib = 1 / (ra + eps), 1 / (rb + eps)
+    diff = a * ia - b * ib
+    dabs = a.abs() * ia + b.abs() * ib
+    d = (wv * diff * diff).sum(1).mean((1, 2))
+    da = (wv.abs() * dabs * dabs).sum(1).mean((1, 2))
+    gs = 2 * gout.double().reshape(-1, 1, 1, 1) / hw
+    t, ta = wv * diff, wv.abs() * dabs
+    res = [d, da]
+    for f, r, i, sign in ((a, ra, ia, 1.0), (b, rb, ib, -1.0)):
+        live = r > 0
+        rr = torch.where(live, r, torch.ones_like(r))
+        kf = (t * f).sum(1, keepdim=True) * i * i / rr
+        ka = (ta * f.abs()).sum(1, keepdim=True) * i * i / rr
+        res.append(torch.where(live, sign * gs * (t * i - f * kf), torch.zeros_like(f)))
+        res.append(torch.where(live, gs.abs() * (ta * i + f.abs() * ka), torch.zeros_like(f)))
+    return res
 
 
 # ======================================================================================== planner restatements (no GPU)

@@ -17,55 +17,20 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from fp64_contract import DEV, SQRT2, blur_plan, ceil_div, finish_depth, lrelu64, randn, rowwise_c, seeded, slope_gain
+from fp64_contract import (DEV, SQRT2, blur_k, blur_plan, ceil_div, check_once, check_sum, cl, distance64, distance_c_terms,
+                           distance_forward_c, finish_depth, fir64, lrelu64, randn, rowwise_c, seeded, slope_gain)
 from oracle import stylegan2_ops as so
-from oracle.rounding import assert_fp32_sum, assert_rounded_once
 
 pytestmark = pytest.mark.gpu
-CL = torch.channels_last
 BF = torch.bfloat16
 CS = [64, 192, 512]                   # 192: a non-power-of-two multiple of the bf16 blur multiple (64)
 SPATIAL = [(4, 4), (9, 9), (33, 29)]
-
-
-def check_once(y, ref, a, k, what, extra=None):
-    ulps, k_obs = assert_rounded_once(y, ref, a, k, what, extra)
-    print("[contract] %s: %.4f ulp, k_obs=%.2f (k=%g)" % (what, ulps, k_obs, k))
-
-
-def check_sum(y, ref, a, c, what, extra=None):
-    r = assert_fp32_sum(y, ref, a, c, what, extra)
-    print("[contract] %s: c_obs=%.2f (c=%d)" % (what, r, c))
-
-
-def cl(t):
-    return t.contiguous(memory_format=CL)
-
-
-def fir64(x, k, pad):
-    """upfirdn2d(up = down = 1) in float64: TRUE convolution with `k` (upfirdn2d.py:185-187), pad = (x0, x1, y0, y1)."""
-    xp = F.pad(x, list(pad))
-    kh, kw = k.shape
-    oh, ow = xp.shape[2] - kh + 1, xp.shape[3] - kw + 1
-    kf = torch.flip(k.double(), [0, 1]).tolist()
-    out = torch.zeros(x.shape[0], x.shape[1], oh, ow, dtype=torch.float64, device=x.device)
-    for a in range(kh):
-        for b in range(kw):
-            out += kf[a][b] * xp[:, :, a:a + oh, b:b + ow]
-    return out
 
 
 # ------------------------------------------------------------------------------------------------ launch geometry -> c
 def _sm():
     from gangealing_b200 import _lib
     return _lib.sm_count()
-
-
-def blur_k(kernel):
-    """fp32 roundings of one blurred value: separable = 4 horizontal + 4 vertical products/sums + the factorised column
-    taps (col / pivot); otherwise 16 fused multiply-adds."""
-    from gangealing_b200 import _lib
-    return 9 if _lib.filter_is_separable(kernel) else 16
 
 
 def filt(kind, gain=1.0):
@@ -292,56 +257,11 @@ def test_styled_tail_backward_nhwc(shape, slope):
 
 
 # ================================================================================================ perceptual front end
-def distance_c_terms(c):
-    """(S, e_ia, TRIPS, L): S = roundings of a pixel's sum of squares (a lane's 4*TRIPS fmas + log2(L) butterfly steps),
-    e_ia = roundings in 1/(sqrt(S) + eps) (S/2 through the square root, sqrt, + eps, the division)."""
-    c4 = c // 4
-    L = min(32, c4)
-    trips = c4 // L
-    s = 4 * trips + int(math.log2(L))
-    return s, s / 2 + 3, trips, L
-
-
-def distance_forward_c(n, c, hw):
-    """distance value: 2*(e_ia + 2) for the squared normalised difference, a lane's fmas and its pixels (chunk / groups),
-    the warp sum (5), the CTA's 8 warps, *1/HW (2), the finish kernel's K partials."""
-    s, e_ia, trips, L = distance_c_terms(c)
-    groups = 256 // L
-    k = max(1, min(ceil_div(8 * _sm(), n), ceil_div(hw, 2 * groups), 64))
-    chunk = ceil_div(hw, k)
-    return int(math.ceil(2 * (e_ia + 2) + 4 * trips + ceil_div(chunk, groups) + 5 + 8 + 2 + ceil_div(hw, chunk)))
-
-
 def distance_backward_k(c):
     """g = gs*(t*ia - a*ka), t = w*(a*ia - b*ib), ka = (sum t*a)*ia*ia/ra: the sums S twice, the inverse norm four times
     over (e_ia each) and ~16 products, differences and the 2*g/HW scale."""
     s, e_ia, _, _ = distance_c_terms(c)
     return int(math.ceil(2 * s + 4 * e_ia + 16))
-
-
-def distance64(a, b, w, gout, eps=1e-10):
-    """float64 feature distance of the stored maps a, b (N, C, H, W), its value on absolute values, and the gradients with
-    their absolute-value counterparts.  A pixel whose map is all zero gets gradient 0 (csrc/lpips.cu)."""
-    hw = a.shape[2] * a.shape[3]
-    wv = w.double().reshape(1, -1, 1, 1) if w is not None else torch.ones(1, a.shape[1], 1, 1, dtype=torch.float64, device=a.device)
-    ra = a.square().sum(1, keepdim=True).sqrt()
-    rb = b.square().sum(1, keepdim=True).sqrt()
-    ia, ib = 1 / (ra + eps), 1 / (rb + eps)
-    diff = a * ia - b * ib
-    dabs = a.abs() * ia + b.abs() * ib
-    d = (wv * diff * diff).sum(1).mean((1, 2))
-    da = (wv.abs() * dabs * dabs).sum(1).mean((1, 2))
-    gs = 2 * gout.double().reshape(-1, 1, 1, 1) / hw
-    t, ta = wv * diff, wv.abs() * dabs
-    res = [d, da]
-    for f, r, i, sign in ((a, ra, ia, 1.0), (b, rb, ib, -1.0)):
-        live = r > 0
-        rr = torch.where(live, r, torch.ones_like(r))
-        kf = (t * f).sum(1, keepdim=True) * i * i / rr
-        ka = (ta * f.abs()).sum(1, keepdim=True) * i * i / rr
-        res.append(torch.where(live, sign * gs * (t * i - f * kf), torch.zeros_like(f)))
-        res.append(torch.where(live, gs.abs() * (ta * i + f.abs() * ka), torch.zeros_like(f)))
-    return res
 
 
 @pytest.mark.parametrize("c", [4, 8, 16, 32, 64, 128, 256, 384, 512, 768, 1024])

@@ -2,18 +2,16 @@
 and the congealing animation with dense point tracking, against the reference fixture (oracle/make_golden_vis.py), the
 float64 oracle (oracle/vis.py) and the reference's per-frame composition; the lerped-grid sampler, its frame-mean kernel and
 the windowed point tracker against torch and float64; a 2-rank gloo run; the C ABI's argument checks."""
-import contextlib
-import os
-import sys
-
 import pytest
 import torch
 
-from conftest import ROOT, assert_close, load_golden
+from conftest import load_golden
 from oracle import make_golden_pck as GP
 from oracle import make_golden_vis as GV
 from oracle import opset
 from oracle import vis as OV
+from ranks import run_ranks
+from vis_reference import fp32_stn
 
 DEV = "cuda"
 AVG = [c[0] for c in GV.AVG_CASES]
@@ -112,15 +110,8 @@ def test_average_congealed_image_reproduces_the_reference_fixture():
     assert _rel(oracle, blob["average.image"], _scale(batches)) <= GV.tolerance(iters)
 
 
-def _gloo_worker(rank, world, port, ret):
-    sys.path.insert(0, ROOT)
-    sys.path.insert(0, os.path.join(ROOT, "tests"))
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world), LOCAL_RANK=str(rank))
-    torch.set_num_threads(2)
-    import torch.distributed as dist
+def _gloo_worker(rank, world, ret):
     from gangealing_b200.evaluation import average_congealed_image, congealing_average_frames
-    from gangealing_b200.training import distributed as gdist
-    assert gdist.setup_distributed("gloo")
     t = _mirror(OV.cpu_ops())
     batches = GV.case_batches(GV.AVG_CASES[0][-1])
     with torch.no_grad():
@@ -129,14 +120,11 @@ def _gloo_worker(rank, world, port, ret):
         avg = average_congealed_image(t, batches[rank:rank + 1], 8, output_resolution=GV.RES)
     if rank == 0:
         ret["frames"], ret["avg"] = frames, avg
-    gdist.synchronize()
-    dist.destroy_process_group()
 
 
 @pytest.mark.timeout(900)
 def test_two_rank_gloo_run_equals_the_single_process_result():
     """Rank r congeals batch r; the single process both batches in order."""
-    import torch.multiprocessing as mp
     from gangealing_b200.evaluation import average_congealed_image, congealing_average_frames
     t = _mirror(OV.cpu_ops())
     batches = GV.case_batches(GV.AVG_CASES[0][-1])
@@ -144,18 +132,9 @@ def test_two_rank_gloo_run_equals_the_single_process_result():
         frames = congealing_average_frames(t, batches, 8, length=3, flip_length=3, vis_in_stages=True, stage_flip=True,
                                            output_resolution=GV.RES)
         avg = average_congealed_image(t, batches, 8, output_resolution=GV.RES)
-    ctx = mp.get_context("spawn")
-    with ctx.Manager() as mgr:
-        ret = mgr.dict()
-        port = 35600 + (os.getpid() % 2000)
-        procs = [ctx.Process(target=_gloo_worker, args=(r, 2, port, ret)) for r in range(2)]
-        for p in procs:
-            p.start()
-        for p in procs:
-            p.join(860)
-        assert all(p.exitcode == 0 for p in procs), [p.exitcode for p in procs]
-        assert _rel(ret["frames"], frames) <= 1e-6, _rel(ret["frames"], frames)
-        assert _rel(ret["avg"], avg) <= 1e-6
+    ret = run_ranks(_gloo_worker, 860)
+    assert _rel(ret["frames"], frames) <= 1e-6, _rel(ret["frames"], frames)
+    assert _rel(ret["avg"], avg) <= 1e-6
 
 
 def test_reference_assertions_raise_value_error():
@@ -322,18 +301,6 @@ def test_track_points_lerp_vs_float64_oracle(patch):
     print("patch %d: %d near-tie differences of %d" % (patch, ties, 2 * T * n * p))
 
 
-@contextlib.contextmanager
-def _fp32_stn():
-    """The STN's cuDNN convolutions and matmuls in fp32, not TF32, so that the GPU run can be held to the CPU fixture
-    (as the other fixture tests on the GPU do)."""
-    old = torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32
-    torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
-    try:
-        yield
-    finally:
-        torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = old
-
-
 def _count_images(t):
     seen = [0]
     handle = t.stns[-1].register_forward_hook(lambda m, inp, out: seen.__setitem__(0, seen[0] + inp[0].size(0)))
@@ -351,7 +318,7 @@ def test_average_frames_on_the_gpu(name):
     kw, n_mean, seed = _avg_cfg(blob, name)
     t = _mirror(cuda_ops()).to(DEV)
     batches = [b.to(DEV) for b in GV.case_batches(seed)]
-    with torch.no_grad(), _fp32_stn():
+    with torch.no_grad(), fp32_stn():
         seen, handle = _count_images(t)
         got = congealing_average_frames(t, batches, n_mean, **kw)
         handle.remove()
@@ -372,7 +339,7 @@ def test_smooth_congealing_on_the_gpu(name):
     kw, seed = _smooth_cfg(blob, name)
     t = _mirror(cuda_ops()).to(DEV)
     data = GV.case_batches(seed, 1)[0].to(DEV)
-    with torch.no_grad(), _fp32_stn():
+    with torch.no_grad(), fp32_stn():
         seen, handle = _count_images(t)
         frames, points, unaligned = smooth_congealing(t, data, blob["label_points"], **kw)
         handle.remove()

@@ -7,6 +7,7 @@ import pytest
 import torch
 
 from gangealing_b200 import _lib
+from styled_reference import bf16_tail_contract, dekink, inputs
 
 DEV = "cuda"
 CL = torch.channels_last
@@ -27,9 +28,8 @@ def _unpack(mask, c):
 
 
 def _tail_inputs(shape, blur, with_rgb, with_next, dtype, exact_zero):
-    from test_styled_fused_gpu import _inputs
     n, c, h, w = shape
-    t = _inputs(n, c, h, w, blur, with_rgb, with_next, seed=c + h)
+    t = inputs(n, c, h, w, blur, with_rgb, with_next, seed=c + h)
     if exact_zero:      # every 8th channel is exactly 0 after the activation: raw = bias = 0 and no noise
         t["raw"][:, ::8] = 0
         t["bias"][::8] = 0
@@ -126,15 +126,14 @@ def test_fused_tail_with_constant_styles_equals_the_general_route(shape, blur, w
 @gpu
 @pytest.mark.parametrize("shape,blur,with_rgb,with_next", SHAPES[:7])
 def test_sign_mask_route_meets_the_bf16_storage_contract(shape, blur, with_rgb, with_next):
-    """The float64 contract of tests/test_styled_fused_gpu.py (each stored value rounded once) on the sign-mask route."""
-    from test_styled_fused_gpu import _bf16_tail_contract, _dekink, _inputs
-    t = _dekink(_inputs(*shape, blur, with_rgb, with_next, seed=shape[1] + shape[2]), blur, torch.bfloat16)
+    """The general route's float64 contract (bf16_tail_contract: each stored value rounded once) on the sign-mask route."""
+    t = dekink(inputs(*shape, blur, with_rgb, with_next, seed=shape[1] + shape[2]), blur, torch.bfloat16)
     d = {k: (v.to(DEV) if isinstance(v, torch.Tensor) else v) for k, v in t.items()}
     d["raw"] = d["raw"].to(torch.bfloat16).contiguous(memory_format=CL)
     if d["g_xs"] is not None:
         d["g_xs"] = d["g_xs"].to(torch.bfloat16).contiguous(memory_format=CL)
     xs, rgb, g_raw = _fused(t, d, blur, ("raw",))
-    _bf16_tail_contract(t, blur, xs, rgb, {"raw": g_raw})
+    bf16_tail_contract(t, blur, xs, rgb, {"raw": g_raw})
 
 
 def test_argument_validation_of_the_sign_mask_entry_points():

@@ -1,24 +1,15 @@
 """CPU, world_size 2 over gloo: the data-parallel logic of the train step (per-rank latents, DDP gradient
 all-reduce keeps replicas identical, rank-0 loss reduce)."""
-import os
-import sys
-
 import pytest
 import torch
-import torch.distributed as dist
-import torch.multiprocessing as mp
 
-from conftest import ROOT
+from ranks import run_ranks
 
 
-def _worker(rank, world, port, ret):
-    sys.path.insert(0, ROOT)
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world), LOCAL_RANK=str(rank))
-    torch.set_num_threads(2)
+def _worker(rank, world, ret):
     from oracle import opset
     from gangealing_b200.training import TrainConfig, Trainer
     from gangealing_b200.training import distributed as gdist
-    assert gdist.setup_distributed("gloo")
     cfg = TrainConfig(gen_size=64, flow_size=64, dim_latent=16, n_mlp=1, batch=1, inject=3, seed=3)
     tr = Trainer(cfg, "cpu", ops=opset.cpu_ops(), distributed=True)
     z_probe = torch.randn(2)                      # the per-rank RNG stream differs (train.py:193)
@@ -32,35 +23,20 @@ def _worker(rank, world, port, ret):
         ret["latents_differ"] = bool(not torch.equal(probes[0], probes[1]))
         ret["loss_keys"] = sorted(out.keys())
         ret["loss_finite"] = bool(all(torch.isfinite(v) for v in out.values()))
-    gdist.synchronize()
-    dist.destroy_process_group()
 
 
 @pytest.mark.timeout(600)
 def test_two_rank_data_parallel_step_gloo():
-    ctx = mp.get_context("spawn")
-    with ctx.Manager() as mgr:
-        ret = mgr.dict()
-        port = 29500 + (os.getpid() % 2000)
-        procs = [ctx.Process(target=_worker, args=(r, 2, port, ret)) for r in range(2)]
-        for p in procs:
-            p.start()
-        for p in procs:
-            p.join(560)
-        assert all(p.exitcode == 0 for p in procs), [p.exitcode for p in procs]
-        assert ret["replicas_equal"], "DDP replicas diverged"
-        assert ret["latents_differ"]
-        assert ret["loss_keys"] == ["f", "p", "tv"] and ret["loss_finite"]
+    ret = run_ranks(_worker, 560)
+    assert ret["replicas_equal"], "DDP replicas diverged"
+    assert ret["latents_differ"]
+    assert ret["loss_keys"] == ["f", "p", "tv"] and ret["loss_finite"]
 
 
-def _worker_cluster(rank, world, port, ret):
-    sys.path.insert(0, ROOT)
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world), LOCAL_RANK=str(rank))
-    torch.set_num_threads(2)
+def _worker_cluster(rank, world, ret):
     from oracle import opset
     from gangealing_b200.training import ClassifierTrainer, TrainConfig, Trainer
     from gangealing_b200.training import distributed as gdist
-    assert gdist.setup_distributed("gloo")
     # the exchange helpers on known per-rank values (reference utils/distributed.py:87-100,140-162)
     mine = torch.tensor([1.0 + rank, 10.0 * (rank + 1)])
     mean = gdist.all_reduce_mean(mine)
@@ -84,25 +60,14 @@ def _worker_cluster(rank, world, port, ret):
         ret["cls_equal"] = bool(torch.equal(cls_all[0], cls_all[1]))
         ret["finite"] = bool(all(torch.isfinite(v) for v in out.values()) and torch.isfinite(cout["cross_entropy"]))
         ret["hist"] = sum(float(cout["head_%d" % c]) for c in range(4))
-    gdist.synchronize()
-    dist.destroy_process_group()
 
 
 @pytest.mark.timeout(900)
 def test_two_rank_cluster_step_classifier_step_and_exchange_helpers_gloo():
-    ctx = mp.get_context("spawn")
-    with ctx.Manager() as mgr:
-        ret = mgr.dict()
-        port = 31500 + (os.getpid() % 2000)
-        procs = [ctx.Process(target=_worker_cluster, args=(r, 2, port, ret)) for r in range(2)]
-        for p in procs:
-            p.start()
-        for p in procs:
-            p.join(860)
-        assert all(p.exitcode == 0 for p in procs), [p.exitcode for p in procs]
-        assert ret["mean"] == [1.5, 15.0]
-        assert ret["reduced"] == {"a": 1.5, "b": 15.0}                 # rank 0 holds the mean over ranks
-        assert ret["gathered"] == [[[1.0, 10.0]], [[2.0, 20.0]]]
-        assert ret["stn_equal"], "DDP replicas of the clustering STN diverged"
-        assert ret["cls_equal"], "DDP replicas of the classifier diverged"
-        assert ret["finite"] and abs(ret["hist"] - 1.0) < 1e-6        # rank-0 mean of per-rank histograms still sums to one
+    ret = run_ranks(_worker_cluster, 860)
+    assert ret["mean"] == [1.5, 15.0]
+    assert ret["reduced"] == {"a": 1.5, "b": 15.0}                 # rank 0 holds the mean over ranks
+    assert ret["gathered"] == [[[1.0, 10.0]], [[2.0, 20.0]]]
+    assert ret["stn_equal"], "DDP replicas of the clustering STN diverged"
+    assert ret["cls_equal"], "DDP replicas of the classifier diverged"
+    assert ret["finite"] and abs(ret["hist"] - 1.0) < 1e-6        # rank-0 mean of per-rank histograms still sums to one

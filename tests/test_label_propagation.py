@@ -5,8 +5,6 @@ the fused splat-and-composite grid op (splat_composite_grid, csrc/splat.cu) agai
 uint8 frames are compared pixel by pixel: the STN here and the reference's round their convolutions in different orders,
 so a tracked point may move (see test_congealing_vis.py) and a value near a quantisation step may round the other way.
 At most 0.5 % of the stored pixels may differ, and the count is reported."""
-import contextlib
-
 import pytest
 import torch
 from torchvision.utils import make_grid
@@ -17,6 +15,7 @@ from oracle import make_golden_labels as GL
 from oracle import make_golden_pck as GP
 from oracle import make_golden_vis as GV
 from oracle import opset
+from vis_reference import fp32_stn
 
 DEV = "cuda"
 CASES = [c[0] for c in GL.LABEL_CASES]
@@ -233,16 +232,6 @@ def test_no_points_is_images2grid_bitwise(n):
     assert torch.equal(got, want)
 
 
-@contextlib.contextmanager
-def _fp32_stn():
-    old = torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32
-    torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
-    try:
-        yield
-    finally:
-        torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = old
-
-
 @pytest.mark.gpu
 def test_dense_tracked_label_vs_float64_oracle():
     """A dense label (every pixel of a 40^2 block at resolution 64, overlapping footprints) tracked by smooth_congealing:
@@ -259,7 +248,7 @@ def test_dense_tracked_label_vs_float64_oracle():
     alpha = torch.rand(1, label.size(0), 1, generator=g)
     t = _mirror(cuda_ops()).to(DEV)
     data = GV.case_batches(seed, 1)[0].to(DEV)
-    with torch.no_grad(), _fp32_stn():
+    with torch.no_grad(), fp32_stn():
         frames, points, _ = smooth_congealing(t, data, label, GV.RESOLUTION, length, flip_length, bool(stages),
                                               bool(stage_flip), GV.RES, iters=iters)
     frames, points = frames[flip_length::12], points[::12]
@@ -278,7 +267,7 @@ def test_dense_tracked_label_vs_float64_oracle():
 def test_videos_on_the_gpu_reproduce_the_fixture(name):
     from gangealing_b200.opset import cuda_ops
     blob = load_golden("label_propagation")
-    with _fp32_stn():
+    with fp32_stn():
         videos = _videos(cuda_ops(), blob, name, DEV)
     assert all(v.is_cuda and v.dtype == torch.uint8 for v in videos.values())
     _check_videos(blob, name, videos)
@@ -288,6 +277,6 @@ def test_videos_on_the_gpu_reproduce_the_fixture(name):
 def test_labeled_average_on_the_gpu_reproduces_the_fixture():
     from gangealing_b200.opset import cuda_ops
     blob = load_golden("label_propagation")
-    with _fp32_stn():
+    with fp32_stn():
         got = _average(cuda_ops(), blob, DEV)
     _check_average(blob, got)

@@ -1,18 +1,14 @@
 """CPU: the latent learner's initialisers (reference train.py:228-243).  The Gram-form IncrementalPCA oracle against the
 reference-generated fixture (sklearn), the package's PCA on the oracle op set against the oracle, k-means++ against the
 reference's per-round distances, Trainer.init_target_mode in place, and a 2-rank gloo run."""
-import os
-import sys
-
 import numpy as np
 import pytest
 import torch
-import torch.distributed as dist
-import torch.multiprocessing as mp
 
-from conftest import ROOT, load_golden
+from conftest import load_golden
 from oracle import make_golden_pca as MG
 from oracle import pca as OP
+from ranks import run_ranks
 
 SKLEARN_COMPONENTS = 1e-5     # oracle (float64 batches) vs sklearn (float32 batch centring, float32 first SVD)
 
@@ -97,53 +93,10 @@ def test_assign_buffers_takes_the_package_pca():
     assert torch.equal(ll.coefficients.detach(), torch.arange(2 * k, dtype=torch.float32).reshape(2, k))
 
 
-def kmeans_setup(device, ops):
-    """The fixture's generator, perceptual loss and latents, built with this package's modules."""
-    from oracle import opset
-    from gangealing_b200.stylegan2 import Generator
-    from gangealing_b200.training.perceptual import PerceptualLoss
-    G = MG.kmeans_generator(Generator, ops=ops).to(device)
-    loss = opset.fill_convs_in_order(PerceptualLoss(ops=ops), MG.KMEANS["vgg_seed"]).to(device)
-    if device != "cpu":
-        loss = loss.to(memory_format=torch.channels_last)
-    return G, loss, MG.kmeans_w().to(device)
-
-
-def run_kmeans(device, ops):
-    """kmeans_plusplus with the fixture's draws injected -> (centroids, per-round distances, per-round probabilities)."""
-    from gangealing_b200.training.latent_learner import kmeans_plusplus
-    blob = load_golden("latent_pca")
-    k = MG.KMEANS
-    G, loss, w = kmeans_setup(device, ops)
-    dists, probs = [], []
-
-    def loss_fn(a, b):
-        d = loss(a, b)
-        dists.append(d.detach().reshape(-1).cpu())
-        return d
-
-    draws = blob["kmeans.draws"]
-    with MG.injected_draws(int(draws[0]), [int(v) for v in draws[1:]]):
-        inner = torch.multinomial
-
-        def spy(p, num_samples=1, **kw):       # records each round's probabilities, then returns the stored draw
-            probs.append(p.detach().cpu())
-            return inner(p, num_samples, **kw)
-
-        torch.multinomial = spy
-        try:
-            centroids = kmeans_plusplus(k["num_heads"], k["num_latent"], MG.FixedLatents(G, w), loss_fn, k["inject_index"],
-                                        k["batch_size"])
-        finally:
-            torch.multinomial = inner
-    per_round = -(-k["num_latent"] // k["batch_size"])
-    rounds = torch.stack([torch.cat(dists[r * per_round:(r + 1) * per_round]) for r in range(k["num_heads"] - 1)])
-    return blob, w, centroids, rounds, torch.stack(probs)
-
-
 def test_kmeans_plusplus_on_the_oracle_op_set_matches_the_reference():
     from oracle import opset
-    blob, w, centroids, dists, probs = run_kmeans("cpu", opset.cpu_ops())
+    blob = load_golden("latent_pca")
+    w, centroids, dists, probs = MG.run_kmeans(blob, "cpu", opset.cpu_ops())
     ref_d, ref_p = blob["kmeans.dists"], blob["kmeans.logits"]
     assert dists.shape == ref_d.shape and probs.shape == ref_p.shape
     assert (dists - ref_d).abs().max() <= 1e-4 * ref_d.abs().max()
@@ -184,14 +137,10 @@ def test_init_target_mode_writes_the_reference_initialisation_in_place(heads, nd
         assert torch.equal(ll.coefficients.detach(), torch.zeros(1, ndirs))
 
 
-def _worker(rank, world, port, ret):
-    sys.path.insert(0, ROOT)
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world), LOCAL_RANK=str(rank))
-    torch.set_num_threads(2)
+def _worker(rank, world, ret):
     from oracle import pca as OP_
     from gangealing_b200.training import Trainer
     from gangealing_b200.training import distributed as gdist
-    assert gdist.setup_distributed("gloo")
     tr = Trainer(_small_config(num_heads=2, ndirs=2), "cpu", ops=OP_.cpu_ops(), distributed=True)
     state = torch.random.get_rng_state()
     mine = tr.generator.batch_latent(3000 // world)
@@ -207,22 +156,11 @@ def _worker(rank, world, port, ret):
         ret["mean_err"] = float(np.abs(pca.mean_ - st["mean"]).max())
         ret["seen"] = pca.n_samples_seen_
         ret["ranks_equal"] = bool(torch.equal(params[0], params[1]))
-    gdist.synchronize()
-    dist.destroy_process_group()
 
 
 @pytest.mark.timeout(600)
 def test_two_rank_init_target_mode_equals_the_fit_over_the_gathered_latents_gloo():
-    ctx = mp.get_context("spawn")
-    with ctx.Manager() as mgr:
-        ret = mgr.dict()
-        port = 31500 + (os.getpid() % 2000)
-        procs = [ctx.Process(target=_worker, args=(r, 2, port, ret)) for r in range(2)]
-        for p in procs:
-            p.start()
-        for p in procs:
-            p.join(560)
-        assert all(p.exitcode == 0 for p in procs), [p.exitcode for p in procs]
-        assert ret["seen"] == 3000
-        assert ret["components_err"] <= 1e-10 and ret["mean_err"] <= 1e-12
-        assert ret["ranks_equal"]
+    ret = run_ranks(_worker, 560)
+    assert ret["seen"] == 3000
+    assert ret["components_err"] <= 1e-10 and ret["mean_err"] <= 1e-12
+    assert ret["ranks_equal"]

@@ -121,12 +121,12 @@ def test_device_pca_equals_the_oracle_and_the_reference_fixture():
 
 @pytest.mark.gpu
 def test_kmeans_plusplus_on_the_device_matches_the_reference():
-    from test_latent_pca import run_kmeans
     from gangealing_b200.opset import cuda_ops
+    blob = load_golden("latent_pca")
     old = torch.backends.cudnn.allow_tf32
     torch.backends.cudnn.allow_tf32 = False
     try:
-        blob, w, centroids, dists, probs = run_kmeans(DEV, cuda_ops())
+        w, centroids, dists, probs = MG.run_kmeans(blob, DEV, cuda_ops())
     finally:
         torch.backends.cudnn.allow_tf32 = old
     ref_d, ref_p = blob["kmeans.dists"], blob["kmeans.logits"]

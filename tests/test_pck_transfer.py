@@ -9,16 +9,14 @@ end against the CPU oracle op set and the fixture; CUDA-graph replay and run-to-
 Comparisons exempt near-ties by one rule (oracle.pck.*_near_ties): a nearest neighbour whose second-best float64 distance
 lies within the rounding band of the best, an error within 1e-4 px of a threshold (scaled up where the grids themselves
 differ), and a flip pick whose two smallest smoothness sums lie within rounding.  The tests bound the exempt share."""
-import os
-import sys
-
 import pytest
 import torch
 
-from conftest import ROOT, assert_close, load_golden
+from conftest import assert_close, load_golden
 from oracle import make_golden_pck as G
 from oracle import opset
 from oracle import pck as OP
+from ranks import run_ranks
 
 DEV = "cuda"
 CASES = ("iters1_border_both", "iters3_reflection_oneway")
@@ -136,17 +134,9 @@ def test_single_forward_evaluator_equals_the_8n_composition_on_fresh_inputs():
     assert 0 < counts.min() and counts.max() < seen
 
 
-def _gloo_worker(rank, world, port, ret):
-    sys.path.insert(0, ROOT)
-    sys.path.insert(0, os.path.join(ROOT, "tests"))
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world), LOCAL_RANK=str(rank))
-    torch.set_num_threads(2)
-    import torch.distributed as dist
-    from conftest import load_golden as lg
+def _gloo_worker(rank, world, ret):
     from gangealing_b200.evaluation import pck_transfer
-    from gangealing_b200.training import distributed as gdist
-    assert gdist.setup_distributed("gloo")
-    blob = lg("pck_transfer")
+    blob = load_golden("pck_transfer")
     kw, both, _, seed = _cfg(blob, CASES[0])
     t = _mirror(OP.cpu_ops())
     # rank r sees the stored batches from batch r on: an uneven split of 11 pairs (6 + 5)
@@ -157,13 +147,10 @@ def _gloo_worker(rank, world, port, ret):
                        permutation=blob["permutation"].tolist(), **kw)
     if rank == 0:
         ret["pck"] = got.tolist()
-    gdist.synchronize()
-    dist.destroy_process_group()
 
 
 @pytest.mark.timeout(600)
 def test_two_rank_gloo_run_equals_the_single_process_result():
-    import torch.multiprocessing as mp
     from gangealing_b200.evaluation import pck_transfer
     blob = load_golden("pck_transfer")
     kw, both, _, seed = _cfg(blob, CASES[0])
@@ -171,17 +158,7 @@ def test_two_rank_gloo_run_equals_the_single_process_result():
     # one process over the same pairs: batch 0 (6 pairs) then the first 5 pairs of batch 1
     single = pck_transfer(t, G.case_loader(blob, CASES[0], seed), OP.ALPHAS, num_pairs=11, device="cpu",
                           transfer_both_ways=both, permutation=blob["permutation"].tolist(), **kw)
-    ctx = mp.get_context("spawn")
-    with ctx.Manager() as mgr:
-        ret = mgr.dict()
-        port = 33500 + (os.getpid() % 2000)
-        procs = [ctx.Process(target=_gloo_worker, args=(r, 2, port, ret)) for r in range(2)]
-        for p in procs:
-            p.start()
-        for p in procs:
-            p.join(560)
-        assert all(p.exitcode == 0 for p in procs), [p.exitcode for p in procs]
-        assert ret["pck"] == single.tolist()
+    assert run_ranks(_gloo_worker, 560)["pck"] == single.tolist()
 
 
 def test_abi_rejects_bad_arguments():

@@ -4,6 +4,7 @@ import pytest
 import torch
 
 from conftest import assert_close, golden_cases, load_golden
+from fp64_contract import check_once, check_sum, distance64, distance_forward_c
 from oracle.perceptual import feature_distance_ref
 
 DEV = "cuda"
@@ -125,7 +126,6 @@ def test_fused_kernels_match_oracle(shape):
     # planar (NCHW) and half-precision maps are converted to the kernel's layout, never evaluated with tensor ops
     assert_close(feature_distance(f0.to(DEV), f1.to(DEV)), ro, rtol=1e-5, what="NCHW input")
     # bf16 maps: the fp32 value against float64 on the stored maps, at the accuracy of the kernel's fp32 sums
-    from test_bf16_storage_gpu import check_sum, distance64, distance_forward_c
     xb, yb = x.detach().bfloat16(), y.detach().bfloat16()
     d, da = distance64(xb.double(), yb.double(), None, go.to(DEV))[:2]
     check_sum(feature_distance(xb, yb).reshape(-1), d, da, distance_forward_c(shape[0], shape[1], shape[2] * shape[3]),
@@ -183,7 +183,6 @@ def test_bias_relu_pool_matches_the_aten_sequence_of_the_reference_backbone(dtyp
     if exact:
         assert torch.equal(y.float().cpu(), y_ref.detach().float()) and torch.equal(p.float().cpu(), p_ref.detach().float())
     else:   # bf16: relu(raw + bias) rounded once (one fp32 add), the pool takes the max of the stored values
-        from test_bf16_storage_gpu import check_once
         check_once(y, torch.relu(raw.double() + bias.double().reshape(1, -1, 1, 1)),
                    raw.double().abs() + bias.double().abs().reshape(1, -1, 1, 1), 1, "relu(raw + bias)")
         assert torch.equal(p.float().cpu(), torch.nn.functional.max_pool2d(y.detach().float().cpu(), 2, 2))
@@ -194,7 +193,6 @@ def test_bias_relu_pool_matches_the_aten_sequence_of_the_reference_backbone(dtyp
             assert torch.equal(gb.cpu(), ga)
         assert_close(gb, ga, rtol=1e-6, what="gradient")
     else:         # bf16 random data: the arg-max decided on the STORED y, the sum g_y + g_pooled rounded once
-        from test_bf16_storage_gpu import check_once
         y64 = y.detach().double().cpu()
         win = y64.reshape(n, c, h // 2, 2, w // 2, 2).permute(0, 1, 2, 4, 3, 5).reshape(n, c, h // 2, w // 2, 4)
         first = torch.nn.functional.one_hot(win.argmax(-1), 4).double()   # argmax: the first maximum

@@ -33,8 +33,8 @@ import pytest
 import torch
 
 from fp64_contract import (BF16, CODE, DEV, F16, F32, H100_SMS, SHORT, SQRT2, TNAME, VEC, Worst, assert_routes_reached,
-                           at_offset, ceil_div, f32, finish_depth, launched, library, lrelu64, nan_at, randn, rowwise_c,
-                           rowwise_geometry, saved_output, seeded, slope_gain)
+                           at_offset, ceil_div, cl, f32, finish_depth, launched, library, lrelu64, nan_at, randn, rowwise_c,
+                           rowwise_geometry, run_fresh, saved_output, seeded, slope_gain)
 
 
 # ======================================================================================== planner restatement (no GPU)
@@ -520,10 +520,6 @@ def test_noise_bias_act_scalar_grid_stride(dt):
 
 
 # ---------------------------------------------------------------------------------------------- channels-last family
-def cl(t):
-    return t.contiguous(memory_format=torch.channels_last)
-
-
 def nhwc_shape(n, c, hw):
     """(N, C, H, W) with H * W = hw and H, W > 1 where possible (so the tensor is unambiguously channels-last)."""
     h = next((d for d in range(2, int(hw ** 0.5) + 1) if hw % d == 0), 1)
@@ -752,21 +748,8 @@ KERNELS = re.compile(r"(rowwise_nchw_rows_kernel|rowwise_nchw_kernel|row_finish_
 @pytest.mark.gpu
 def test_routing_matches_the_restatement():
     """Every distinct route of the cases above launches the kernels (names, template arguments, order) the restatement
-    names.  The check runs in a fresh interpreter: in a process that has already run the rest of the GPU suite, the
-    profiler's sessions recorded the runtime calls (cudaLaunchKernel) but no kernel activity, so the names could not be
-    read there."""
-    import os
-    import subprocess
-    import sys
-    here = os.path.dirname(os.path.abspath(__file__))
-    root = os.path.dirname(here)
-    env = dict(os.environ)
-    env["PYTHONPATH"] = os.pathsep.join([here, root] + ([env["PYTHONPATH"]] if env.get("PYTHONPATH") else []))
-    flags = ["-s"] if sys.flags.no_user_site else []
-    proc = subprocess.run([sys.executable] + flags + ["-c", "import test_rowwise_family_gpu as t; t.check_routing()"],
-                          cwd=root, env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=900)
-    print(proc.stdout)
-    assert proc.returncode == 0, "routing check failed:\n%s" % proc.stdout[-6000:]
+    names."""
+    run_fresh("test_rowwise_family_gpu", "check_routing")
 
 
 def check_routing():

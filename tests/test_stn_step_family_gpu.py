@@ -40,7 +40,7 @@ import torch
 import torch.nn.functional as F
 
 from fp64_contract import (BF16, CODE, DEV, F32, H100_SMS, Worst, assert_routes_reached, ceil_div, f32, grid_for, launched,
-                           library, seeded)
+                           library, run_fresh, seeded)
 from oracle.rounding import U32, assert_fp32_sum
 
 THREADS = 256
@@ -941,20 +941,8 @@ KERNELS = re.compile(r"(flow_compose_fwd_kernel|flow_compose_bwd_kernel|flow_low
 @pytest.mark.gpu
 def test_launch_sets_match_the_restatement():
     """Each flow-backward output subset launches exactly the restated kernels, the TV forward launches tv_fwd then
-    tv_finish, and an Adam step with no CTAs launches only the tick.  In a fresh interpreter: in a process that has
-    already run other GPU tests, torch.profiler can record the runtime calls without any kernel activity."""
-    import os
-    import subprocess
-    import sys
-    here = os.path.dirname(os.path.abspath(__file__))
-    root = os.path.dirname(here)
-    env = dict(os.environ)
-    env["PYTHONPATH"] = os.pathsep.join([here, root] + ([env["PYTHONPATH"]] if env.get("PYTHONPATH") else []))
-    flags = ["-s"] if sys.flags.no_user_site else []
-    proc = subprocess.run([sys.executable] + flags + ["-c", "import test_stn_step_family_gpu as t; t.check_launch_sets()"],
-                          cwd=root, env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=900)
-    print(proc.stdout)
-    assert proc.returncode == 0, "launch-set check failed:\n%s" % proc.stdout[-6000:]
+    tv_finish, and an Adam step with no CTAs launches only the tick."""
+    run_fresh("test_stn_step_family_gpu", "check_launch_sets")
 
 
 def check_launch_sets():

@@ -30,7 +30,8 @@ import pytest
 import torch
 
 from fp64_contract import (BF16, CODE, DEV, F32, H100_SMS, SHORT, SQRT2, TNAME, VEC, Worst, assert_routes_reached,
-                           ceil_div, f32, launched, library, nan_at, rowwise_c, rowwise_geometry, saved_output, seeded)
+                           ceil_div, f32, launched, library, nan_at, rowwise_c, rowwise_geometry, run_fresh, saved_output,
+                           seeded)
 from oracle.rounding import U32
 
 UNROLL = {F32: 4, BF16: 2}        # pixels in flight per thread in the backward's unrolled loop
@@ -708,20 +709,8 @@ KERNELS = re.compile(r"(styled_tail_nhwc_kernel|styled_tail_bwd_nhwc_kernel|nhwc
 @pytest.mark.gpu
 def test_routing_matches_the_restatement():
     """Every distinct route of the cases above launches the kernels (names, template arguments, number of finish
-    launches) the restatement names.  The check runs in a fresh interpreter: in a process that has already run other GPU
-    tests, torch.profiler can record the runtime calls without any kernel activity."""
-    import os
-    import subprocess
-    import sys
-    here = os.path.dirname(os.path.abspath(__file__))
-    root = os.path.dirname(here)
-    env = dict(os.environ)
-    env["PYTHONPATH"] = os.pathsep.join([here, root] + ([env["PYTHONPATH"]] if env.get("PYTHONPATH") else []))
-    flags = ["-s"] if sys.flags.no_user_site else []
-    proc = subprocess.run([sys.executable] + flags + ["-c", "import test_styled_tail_family_gpu as t; t.check_routing()"],
-                          cwd=root, env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=900)
-    print(proc.stdout)
-    assert proc.returncode == 0, "routing check failed:\n%s" % proc.stdout[-6000:]
+    launches) the restatement names."""
+    run_fresh("test_styled_tail_family_gpu", "check_routing")
 
 
 def check_routing():

@@ -7,8 +7,11 @@ import sys
 import pytest
 import torch
 
+from oracle import make_golden_training_vis as GT
 from oracle import opset
 from oracle import training_vis as OT
+from ranks import run_ranks
+from vis_reference import DIFFER_BOUND, case_grids, compare_to_fixture, mirror_models
 
 CPU = opset.cpu_ops()
 OPS = OT.cpu_ops()
@@ -194,67 +197,6 @@ def test_compat_registers_flow_to_image():
 
 
 # ------------------------------------------------------------------------------------ the reference's own grids
-from oracle import make_golden_training_vis as GT  # noqa: E402
-
-DIFFER_BOUND = 0.005
-
-
-def mirror_models(ops, k, flips, device="cpu"):
-    """This repo's generator, STN, latent learner and classifier with the fixture's seeded weights, as the duck-typed
-    trainer / classifier trainer training_visuals and classifier_visuals read."""
-    import types
-    from oracle.make_golden import _mse, classifier_setup
-    from gangealing_b200.cluster_classifier import ResnetClassifier
-    from gangealing_b200.stn import BilinearDownsample, get_stn
-    from gangealing_b200.stylegan2 import Generator
-    from gangealing_b200.training import DirectionInterpolator
-
-    def with_ops(cls):
-        return lambda *a, **kw: cls(*a, ops=ops, **kw)
-    mods = dict(Generator=with_ops(Generator), get_stn=with_ops(get_stn), DirectionInterpolator=DirectionInterpolator,
-                ResnetClassifier=with_ops(ResnetClassifier), BilinearDownsample=with_ops(BilinearDownsample))
-    g, stn, ll, cls, resize, _ = classifier_setup(mods, heads=k, flips=flips)
-    g, stn, ll, cls, resize = [m.to(device) for m in (g, stn, ll, cls, resize)]
-    cfg = types.SimpleNamespace(num_heads=k, flips=flips, padding_mode=GT.PADDING)
-    trainer = types.SimpleNamespace(cfg=cfg, generator=g, t_ema=stn, ll=ll, ll_module=ll, loss_fn=_mse, resize_fake2stn=resize,
-                                    psi_t=GT.PSI, device=device)
-    return trainer, types.SimpleNamespace(trainer=trainer, classifier=cls)
-
-
-def case_grids(ops, case, device="cpu", vis_ops=None):
-    from gangealing_b200.training import visuals as V
-    name, k, flips, n_mean, vb, kind = case
-    trainer, ct = mirror_models(ops, k, flips, device)
-    z, big_z, reals, loader = [x.to(device) if torch.is_tensor(x) else [b.to(device) for b in x] for x in GT.inputs()]
-    torch.manual_seed(GT.NOISE_SEED)
-    if kind == "classifier":
-        return V.classifier_visuals(ct, loader, n_mean, GT.N_SAMPLE, ops=vis_ops)
-    return V.training_visuals(trainer, z, big_z if k > 1 else None, reals, loader, n_mean, GT.N_SAMPLE, vb, ops=vis_ops)
-
-
-def compare_to_fixture(grids, blob, case, skip=()):
-    """Every grid's shape and sums, and its stored pixels: at most 0.5 % differ, each by one step (pixels that pass
-    through the mirror STN / generator may land on the other side of a quantisation step).  -> (differing, total)."""
-    names = GT.grid_names(blob, case)
-    assert sorted(grids) == names, "%s: grids %s, the reference logs %s" % (case, sorted(grids), names)
-    differ = total = 0
-    for name in names:
-        got = grids[name].cpu()
-        assert tuple(got.shape) == tuple(blob["%s.%s.shape" % (case, name)].tolist()), "%s.%s shape" % (case, name)
-        if name in skip:
-            continue
-        want = blob["%s.%s" % (case, name)]
-        d = (GT.decimate(name, got).long() - want.long()).abs()
-        n = int((d > 0).sum())
-        print("%s.%s: %d of %d stored values differ (max %d)" % (case, name, n, d.numel(), int(d.max())))
-        assert int(d.max()) <= 1 and n <= DIFFER_BOUND * d.numel(), "%s.%s: %d values differ, max %d" % (case, name, n,
-                                                                                                        int(d.max()))
-        pixels = got.size(0) * got.size(1)
-        assert (got.long().sum((0, 1)) - blob["%s.%s.sums" % (case, name)]).abs().max() <= DIFFER_BOUND * pixels
-        differ, total = differ + n, total + d.numel()
-    return differ, total
-
-
 @pytest.mark.parametrize("case", GT.CASES, ids=[c[0] for c in GT.CASES])
 def test_api_reproduces_the_reference_grids_on_the_cpu_op_set(case):
     from conftest import load_golden
@@ -278,16 +220,10 @@ def test_oracle_restatements_reproduce_the_reference_flow_and_mean_grids():
 
 
 # --------------------------------------------------------------------------------------------- two ranks over gloo
-def _worker_two_ranks(rank, world, port, ret):
-    from conftest import ROOT
-    sys.path.insert(0, ROOT)
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world), LOCAL_RANK=str(rank))
-    torch.set_num_threads(2)
-    import torch.distributed as tdist
+def _worker_two_ranks(rank, world, ret):
     from gangealing_b200.training import Trainer
     from gangealing_b200.training import distributed as gdist
     from gangealing_b200.training import visuals as V
-    assert gdist.setup_distributed("gloo")
     tr = Trainer(_cfg(2, True), "cpu", ops=CPU)
     z, big_z, _, loader = _inputs(10 + rank)               # each rank its own fakes and real batches
     big_z = big_z[:4]                                       # n_mean // world = 4 fakes per rank, batches of 3: 3 + 1
@@ -313,30 +249,18 @@ def _worker_two_ranks(rank, world, port, ret):
         ret["counts"] = counts
     else:
         ret["rank1_grids"] = len(grids)
-    gdist.synchronize()
-    tdist.destroy_process_group()
 
 
 @pytest.mark.timeout(600)
 def test_two_rank_means_follow_the_reference_formulas_gloo():
     """world 2: the per-cluster means divide the ranks' summed sums by the ranks' summed max(count, n_sample), the real
     means by all images seen on both ranks; rank 0 returns the grids, rank 1 none."""
-    import torch.multiprocessing as mp
-    ctx = mp.get_context("spawn")
-    with ctx.Manager() as mgr:
-        ret = mgr.dict()
-        port = 29500 + (os.getpid() + 777) % 2000
-        procs = [ctx.Process(target=_worker_two_ranks, args=(r, 2, port, ret)) for r in range(2)]
-        for p in procs:
-            p.start()
-        for p in procs:
-            p.join(560)
-        assert all(p.exitcode == 0 for p in procs), [p.exitcode for p in procs]
-        grids = ret["grids"]
-        assert ret["rank1_grids"] == 0
-        assert min(ret["counts"]) < 4
-        for name, means in (("mean_generated_EMA_transformed_assigned", ret["fake_means"]),
-                            ("mean_EMA_transformed_real_sample", ret["real_means"])):
-            want = OT.images2grid(means, 1, None, scale_each=True)
-            d = (grids[name].long() - want.long()).abs()
-            assert int(d.max()) <= 1 and int((d > 0).sum()) <= DIFFER_BOUND * d.numel(), name
+    ret = run_ranks(_worker_two_ranks, 560)
+    grids = ret["grids"]
+    assert ret["rank1_grids"] == 0
+    assert min(ret["counts"]) < 4
+    for name, means in (("mean_generated_EMA_transformed_assigned", ret["fake_means"]),
+                        ("mean_EMA_transformed_real_sample", ret["real_means"])):
+        want = OT.images2grid(means, 1, None, scale_each=True)
+        d = (grids[name].long() - want.long()).abs()
+        assert int(d.max()) <= 1 and int((d > 0).sum()) <= DIFFER_BOUND * d.numel(), name

@@ -5,6 +5,7 @@ import torch
 
 from oracle import make_golden_training_vis as GT
 from oracle import training_vis as OT
+from vis_reference import case_grids, compare_to_fixture, mirror_models
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -178,7 +179,6 @@ def test_visuals_reproduce_the_reference_grids_on_the_gpu(case, fp32_convolution
     compared with the reference's: a difference is allowed only at a near-tie (the two best losses within 1e-4
     relative), and the counts are reported."""
     from conftest import load_golden
-    from test_training_vis import case_grids, compare_to_fixture, mirror_models
     blob = load_golden("training_vis")
     name, k, flips = case[:3]
     differ, total = compare_to_fixture(case_grids(None, case, DEV), blob, name)

@@ -42,7 +42,7 @@ import pytest
 import torch
 
 from fp64_contract import (BF16, CODE, DEV, F16, F32, H100_SMS, SHORT, TNAME, Worst, assert_routes_reached, ceil_div, f32,
-                           grid_for, launched, library, nan_at, seeded)
+                           grid_for, launched, library, nan_at, run_fresh, seeded)
 from oracle import sampling as S
 from oracle.rounding import assert_fp32_sum, assert_rounded_once
 from warp_reference import (LN2, _edge_grid, _take, argmax_targets, bilinear_slopes, blend, blend_abs, build_stack,
@@ -942,20 +942,8 @@ def _tb(flag):
 def test_each_entry_launches_its_labelled_instantiation():
     """Each entry launches exactly the instantiation its case is labelled with: warp_compose_fwd_kernel<T, MIP, MODE>,
     warp_lerp_mean_kernel<T, MIP, C>, warp_bwd_kernel<T, MIP> and sample_indices_kernel (one profiler session per
-    dtype x MIP, the calls in order).  In a fresh interpreter, as test_stn_step_family_gpu's launch test: in a process that
-    has already run other GPU tests, torch.profiler can record the runtime calls without any kernel activity."""
-    import os
-    import subprocess
-    import sys
-    here = os.path.dirname(os.path.abspath(__file__))
-    root = os.path.dirname(here)
-    env = dict(os.environ)
-    env["PYTHONPATH"] = os.pathsep.join([here, root] + ([env["PYTHONPATH"]] if env.get("PYTHONPATH") else []))
-    flags = ["-s"] if sys.flags.no_user_site else []
-    proc = subprocess.run([sys.executable] + flags + ["-c", "import test_warp_family_gpu as t; t.check_launches()"],
-                          cwd=root, env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=900)
-    print(proc.stdout)
-    assert proc.returncode == 0, "launch check failed:\n%s" % proc.stdout[-6000:]
+    dtype x MIP, the calls in order)."""
+    run_fresh("test_warp_family_gpu", "check_launches")
 
 
 def check_launches():

@@ -292,6 +292,7 @@ int check_args(int64_t N, int C, int H, int W, int levels, int width, const floa
   if (levels < 1) return fail(GG_ERR_BAD_ARG, "%s: levels must be >= 1 (got %d)", what, levels);
   if (N > 65535) return fail(GG_ERR_UNSUPPORTED, "%s: batch > 65535", what);
   if (levels > 1) {
+    if (H > 65535 * kTH) return fail(GG_ERR_UNSUPPORTED, "%s: height > %d (65535 row tiles of %d)", what, 65535 * kTH, kTH);
     if (!taps) return fail(GG_ERR_BAD_ARG, "%s: null taps", what);
     if (width < 1 || width % 2 == 0) return fail(GG_ERR_BAD_ARG, "%s: tap width must be odd and positive (got %d)", what, width);
     if (width > kMaxWidth) return fail(GG_ERR_UNSUPPORTED, "%s: tap width %d exceeds the cap of %d", what, width, kMaxWidth);

@@ -249,8 +249,11 @@ static int splat_impl(float* out, void* workspace, const float* input, const flo
   SplatParams p;
   p.n = N; p.points = P; p.c = C; p.h = H; p.w = W;
   p.slots = ((C + 1) + 3) / 4 * 4;
-  if (lk && (p.slots != 4 || static_cast<int64_t>(H) * W >= 0x7fffffffLL))
+  if (lk && p.slots != 4)
     return fail(GG_ERR_UNSUPPORTED, "splat2d_lookup: the fused lookup serves C <= 3 (the call sites splat RGB colours or a 1-channel mask)");
+  // only the direct kernel performs the lookup, and it addresses the accumulators with 32-bit pixel offsets
+  if (lk && static_cast<int64_t>(H) * W * p.slots >= 0x7fffffffLL)
+    return fail(GG_ERR_UNSUPPORTED, "splat2d_lookup: H * W * 4 accumulator slots must stay below 2^31 (the fused lookup's scatter)");
   cudaError_t e = cudaMemsetAsync(workspace, 0, static_cast<size_t>(gg_splat2d_workspace(N, C, H, W)), st);
   if (e != cudaSuccess) return cuda_fail(e, "splat2d workspace memset");
   float* acc = static_cast<float*>(workspace);

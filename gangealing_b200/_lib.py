@@ -79,6 +79,7 @@ SIGNATURES = {
     "gg_splat2d_forward": (_I, [_P] * 6 + [_L, _L, _I, _I, _I, _I, _P]),
     "gg_splat_composite_grid_workspace": (_L, [_L, _L, _I, _I]),
     "gg_splat_composite_grid": (_I, [_P, _P, _L, _P, _P, _P, _P, _F, _F, _L, _L, _L, _I, _I, _I, _I, _I, _I, _P]),
+    "gg_splat_lookup_composite_grid": (_I, [_P] * 10 + [_F, _F, _L, _L] + [_I] * 9 + [_P]),
     "gg_flow_compose_forward": (_I, [_P] * 7 + [_L, _I, _I, _I, _P]),
     "gg_flow_compose_backward": (_I, [_P] * 10 + [_L, _I, _I, _I, _P]),
     "gg_mipmap_warp_backward": (_I, [_P] * 7 + [_I, _L] + [_I] * 6 + [_F, _F, _I, _P]),

@@ -142,18 +142,35 @@ struct GridParams {
   float sigma, opacity;
 };
 
+// LOOKUP (gg_splat_lookup_composite_grid, one frame): the points arrive as query coordinates in the congealed frame,
+// (query_n in {1, N}, P, 2), and are looked up in image n's sampling grid (lookup.cuh), then mirrored where flip[n] is set
+// (reference applications/propagate_to_images.py:64-69: uncongeal_points on the flipped image, x -> (R - 1) - x).
+struct FrameLookup {
+  LookupParams lk;
+  const unsigned char* flip;  // (N,) or null
+  int query_n;                // 1 (broadcast) or N
+};
+
 // One thread per (frame, image, point); the footprint schedule and bounds test of splat_direct_kernel.
-template <bool ALPHA>
+template <bool ALPHA, bool LOOKUP>
 __global__ void __launch_bounds__(64)
 splat_frames_kernel(float* __restrict__ acc, const float* __restrict__ coords, const float* __restrict__ colors,
-                    const float* __restrict__ alpha, GridParams p, int64_t total) {
+                    const float* __restrict__ alpha, GridParams p, int64_t total, FrameLookup fl) {
   constexpr int SLOTS = ALPHA ? 8 : 4;
   const int64_t index = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (index >= total) return;
   const int64_t image = index / p.points;            // (frame, image) within the chunk
   const int64_t pt = index - image * p.points;
   const int64_t n = image % p.n;
-  const float2 xy = __ldg(reinterpret_cast<const float2*>(coords + index * 2));
+  float2 xy;
+  if (LOOKUP) {
+    const float2 q = __ldg(reinterpret_cast<const float2*>(coords + ((fl.query_n == 1 ? 0 : n) * p.points + pt) * 2));
+    xy = lookup_point(fl.lk, n, q.x, q.y);
+    if (fl.flip && fl.flip[n]) xy.x = static_cast<float>(p.r - 1) - xy.x;
+    if (fl.lk.points_out) *reinterpret_cast<float2*>(fl.lk.points_out + index * 2) = xy;
+  } else {
+    xy = __ldg(reinterpret_cast<const float2*>(coords + index * 2));
+  }
   const float x = xy.x, y = xy.y;
   const int h = p.r, w = p.r;
   if (!(x >= 0.f && x < static_cast<float>(w) && y >= 0.f && y < static_cast<float>(h))) return;
@@ -351,11 +368,11 @@ int gg_splat_composite_grid(unsigned char* out, void* workspace, int64_t workspa
       const unsigned sblocks = static_cast<unsigned>((total + 63) / 64);
       const float* pts = points + t0 * N * P * 2;
       if (has_alpha) {
-        splat_frames_kernel<true><<<sblocks, 64, 0, st>>>(acc, pts, colors, alpha, p, total);
+        splat_frames_kernel<true, false><<<sblocks, 64, 0, st>>>(acc, pts, colors, alpha, p, total, FrameLookup{});
         GG_CHECK_LAUNCH("splat_frames launch");
         composite_grid_kernel<true, true><<<blocks, 256, 0, st>>>(o, acc, img, p, pix);
       } else {
-        splat_frames_kernel<false><<<sblocks, 64, 0, st>>>(acc, pts, colors, nullptr, p, total);
+        splat_frames_kernel<false, false><<<sblocks, 64, 0, st>>>(acc, pts, colors, nullptr, p, total, FrameLookup{});
         GG_CHECK_LAUNCH("splat_frames launch");
         composite_grid_kernel<true, false><<<blocks, 256, 0, st>>>(o, acc, img, p, pix);
       }
@@ -364,6 +381,75 @@ int gg_splat_composite_grid(unsigned char* out, void* workspace, int64_t workspa
     }
     GG_CHECK_LAUNCH("composite_grid launch");
   }
+  return GG_OK;
+}
+
+int gg_splat_lookup_composite_grid(unsigned char* out, float* points_out, void* workspace, int64_t workspace_bytes,
+                                   const float* images, const float* grid, const float* query, const unsigned char* flip,
+                                   const float* colors, const float* alpha, float sigma, float opacity, int64_t N, int64_t P,
+                                   int query_n, int C, int R, int grid_h, int grid_w, int nrow, int padding, int colors_n,
+                                   int alpha_n, void* stream) {
+  constexpr int64_t kIntMax = 0x7fffffffLL;
+  if (N < 1 || P < 0 || R < 1 || nrow < 1 || padding < 0 || grid_h < 1 || grid_w < 1)
+    return fail(GG_ERR_BAD_ARG, "splat_lookup_composite_grid: P, padding >= 0 and N, R, nrow, grid_h, grid_w >= 1");
+  if (C != 3) return fail(GG_ERR_BAD_ARG, "splat_lookup_composite_grid: C must be 3 (RGB images and colours)");
+  if (!(sigma > 0.f)) return fail(GG_ERR_BAD_ARG, "splat_lookup_composite_grid: sigma must be > 0");
+  if (!(opacity >= 0.f && opacity <= 1.f))
+    return fail(GG_ERR_BAD_ARG, "splat_lookup_composite_grid: opacity must lie in [0, 1]");
+  if (!out || !images) return fail(GG_ERR_BAD_ARG, "splat_lookup_composite_grid: null output or images");
+  const bool splat = P > 0;
+  const bool has_alpha = alpha != nullptr;
+  if (splat && (!grid || !query || !colors || !workspace))
+    return fail(GG_ERR_BAD_ARG, "splat_lookup_composite_grid: null grid, query, colors or workspace");
+  if (splat && query_n != 1 && query_n != N) return fail(GG_ERR_BAD_ARG, "splat_lookup_composite_grid: query_n must be 1 or N");
+  if (splat && colors_n != 1 && colors_n != N) return fail(GG_ERR_BAD_ARG, "splat_lookup_composite_grid: colors_n must be 1 or N");
+  if (splat && has_alpha && alpha_n != 1 && alpha_n != N)
+    return fail(GG_ERR_BAD_ARG, "splat_lookup_composite_grid: alpha_n must be 1 or N");
+  if (splat && reinterpret_cast<uintptr_t>(workspace) % 16 != 0)
+    return fail(GG_ERR_BAD_ARG, "splat_lookup_composite_grid: workspace must be 16-byte aligned (vector reductions)");
+  if (splat && (reinterpret_cast<uintptr_t>(query) % 8 != 0 || reinterpret_cast<uintptr_t>(grid) % 8 != 0 ||
+                reinterpret_cast<uintptr_t>(points_out) % 8 != 0))
+    return fail(GG_ERR_BAD_ARG, "splat_lookup_composite_grid: query, grid and points_out must be 8-byte aligned");
+  GridParams p;
+  p.n = N; p.points = P; p.r = R;
+  const int slots = has_alpha ? 8 : 4;
+  const int64_t frame_acc = N * R * static_cast<int64_t>(R) * slots;
+  if (!make_grid_layout(p.g, N, R, R, nrow, padding) || frame_acc > kIntMax || N * 3 * R * static_cast<int64_t>(R) > kIntMax ||
+      N * P > kIntMax)
+    return fail(GG_ERR_BAD_ARG, "splat_lookup_composite_grid: the grid, images, accumulators or points exceed 2^31 elements");
+  const int64_t frame_bytes = frame_acc * static_cast<int64_t>(sizeof(float));
+  if (splat && workspace_bytes < frame_bytes)
+    return fail(GG_ERR_BAD_ARG, "splat_lookup_composite_grid: the workspace holds less than the grid's accumulators");
+  p.colors_n = colors_n; p.alpha_n = alpha_n; p.sigma = sigma; p.opacity = opacity;
+  FrameLookup fl;
+  // uncongeal_points' unnormalize(points, R, R): k = (R - 1) / R formed in double and rounded once, m = R - 1
+  fl.lk.grid = grid; fl.lk.gh = grid_h; fl.lk.gw = grid_w;
+  fl.lk.k = static_cast<float>(static_cast<double>(R - 1) / R); fl.lk.m = static_cast<float>(R - 1);
+  fl.lk.points_out = points_out;
+  fl.flip = flip; fl.query_n = query_n;
+  auto st = static_cast<cudaStream_t>(stream);
+  float* acc = static_cast<float*>(workspace);
+  const int64_t pix = static_cast<int64_t>(p.g.hg) * p.g.wg;
+  const unsigned blocks = static_cast<unsigned>((pix + 255) / 256);
+  if (!splat) {
+    composite_grid_kernel<false, false><<<blocks, 256, 0, st>>>(out, nullptr, images, p, pix);
+    GG_CHECK_LAUNCH("composite_grid launch");
+    return GG_OK;
+  }
+  cudaError_t e = cudaMemsetAsync(acc, 0, static_cast<size_t>(frame_bytes), st);
+  if (e != cudaSuccess) return cuda_fail(e, "splat_lookup_composite_grid workspace memset");
+  const int64_t total = N * P;
+  const unsigned sblocks = static_cast<unsigned>((total + 63) / 64);
+  if (has_alpha) {
+    splat_frames_kernel<true, true><<<sblocks, 64, 0, st>>>(acc, query, colors, alpha, p, total, fl);
+    GG_CHECK_LAUNCH("splat_frames lookup launch");
+    composite_grid_kernel<true, true><<<blocks, 256, 0, st>>>(out, acc, images, p, pix);
+  } else {
+    splat_frames_kernel<false, true><<<sblocks, 64, 0, st>>>(acc, query, colors, nullptr, p, total, fl);
+    GG_CHECK_LAUNCH("splat_frames lookup launch");
+    composite_grid_kernel<true, false><<<blocks, 256, 0, st>>>(out, acc, images, p, pix);
+  }
+  GG_CHECK_LAUNCH("composite_grid launch");
   return GG_OK;
 }
 

@@ -22,6 +22,7 @@ def cuda_ops():
         from .splat2d import splat2d_lookup as _splat2d_lookup
         from .splat2d import track_points_lerp as _track_points_lerp
         from .splat2d import splat_composite_grid as _splat_composite_grid
+        from .splat2d import splat_lookup_composite_grid as _splat_lookup_composite_grid
         from .splat2d import laplacian_blend as _laplacian_blend
         from .op import feature_distance as _fd
         from .op import vgg_pool as _vp
@@ -60,6 +61,7 @@ def cuda_ops():
             mipmap_warp_lerp_mean=_smp.mipmap_warp_lerp_mean,   # ... and their per-frame batch sums, frames never written
             track_points_lerp=_track_points_lerp,         # dense point tracking over a stage's frames, one launch
             splat_composite_grid=_splat_composite_grid,   # label propagation: splats + composite + uint8 grid per frame
+            splat_lookup_composite_grid=_splat_lookup_composite_grid,   # edits on real images: lookup + flip + splat + grid
             flow_image_grid=_grids.flow_image_grid,       # training visuals: colour-wheel flow images as a uint8 grid
             image_grid=_grids.image_grid,                 # ... min/max-normalised uint8 grid (per-image ranges)
             cluster_accumulate=_grids.cluster_accumulate,  # ... per-cluster sums of routed images, in order, on the device

@@ -2,10 +2,11 @@
 import torch.nn as nn
 
 from .blend import LaplacianBlender, laplacian_blend, splat_points
-from .functional import nn_argmin, splat2d, splat2d_lookup, splat_composite_grid, track_points_lerp
+from .functional import (nn_argmin, splat2d, splat2d_lookup, splat_composite_grid, splat_lookup_composite_grid,
+                         track_points_lerp)
 
 __all__ = ["Splat2D", "splat2d", "splat2d_lookup", "nn_argmin", "track_points_lerp", "laplacian_blend", "LaplacianBlender",
-           "splat_points", "splat_composite_grid"]
+           "splat_points", "splat_composite_grid", "splat_lookup_composite_grid"]
 
 
 class Splat2D(nn.Module):

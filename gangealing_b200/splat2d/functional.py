@@ -8,7 +8,8 @@ import torch.autograd as ag
 
 from .. import _lib
 
-__all__ = ["splat2d", "splat2d_lookup", "nn_argmin", "track_points_lerp", "splat_composite_grid"]
+__all__ = ["splat2d", "splat2d_lookup", "nn_argmin", "track_points_lerp", "splat_composite_grid",
+           "splat_lookup_composite_grid"]
 
 
 class Splat2DFunction(ag.Function):
@@ -170,3 +171,50 @@ def splat_composite_grid(images, points, colors, alpha_channel, sigma, opacity, 
                                      int(nrow), int(padding), counts[0], counts[1], _lib.stream())
     _lib.check(rc, "gg_splat_composite_grid")
     return out
+
+
+@torch.no_grad()
+def splat_lookup_composite_grid(images, grid, query, flip, colors, alpha_channel, sigma, opacity, nrow, padding=2):
+    """A dense label put on real images (reference applications/propagate_to_images.py:62-73) as one grid:
+    uncongeal_points' lookup of `query` in every image's sampling grid (unnormalised to the images' R), the x mirror
+    (R - 1) - x where the image was flipped, splat_points (alpha blending) and images2grid(nrow, padding, range=(-1, 1)),
+    in one scatter and one composite launch (csrc/splat.cu).
+    images (N, 3, R, R) fp32; grid (N, Hg, Wg, 2) the STN's sampling grids; query (1 or N, P, 2) normalised congealed
+    coordinates; flip (N,) bool or None; colors (N or 1, P, 3) (required) and alpha_channel (N or 1, P, 1) or None.
+    -> ((Hg, Wg, 3) uint8 grid, (N, P, 2) fp32 pixel coordinates on the unflipped images), both on the device."""
+    _lib.require_cuda(images, grid, query, flip, colors, alpha_channel)
+    if images.dim() != 4 or images.size(1) != 3 or images.size(2) != images.size(3):
+        raise RuntimeError("splat_lookup_composite_grid: images must be (N, 3, R, R)")
+    n, _, r, _ = images.shape
+    if grid.dim() != 4 or grid.size(0) != n or grid.size(3) != 2:
+        raise RuntimeError("splat_lookup_composite_grid: grid must be (N, Hg, Wg, 2) with N = %d" % n)
+    if query.dim() != 3 or query.size(0) not in (1, n) or query.size(2) != 2:
+        raise RuntimeError("splat_lookup_composite_grid: query must be (N or 1, P, 2) with N = %d" % n)
+    p = query.size(1)
+    if colors is None:
+        raise ValueError("splat_lookup_composite_grid: colors is required (plotly colour scales are not supported)")
+    counts = []
+    for name, v, c in (("colors", colors, 3), ("alpha_channel", alpha_channel, 1)):
+        if v is not None and (v.dim() != 3 or v.size(0) not in (1, n) or v.size(1) != p or v.size(2) != c):
+            raise RuntimeError("splat_lookup_composite_grid: %s must be (N or 1, P, %d) with N = %d, P = %d" % (name, c, n, p))
+        counts.append(v.size(0) if v is not None else 1)
+    if flip is not None and flip.numel() != n:
+        raise RuntimeError("splat_lookup_composite_grid: flip must hold N = %d values" % n)
+    images, grid, query, colors = [v.float().contiguous() for v in (images, grid, query, colors)]
+    alpha_channel = None if alpha_channel is None else alpha_channel.float().contiguous()
+    flip = None if flip is None else flip.reshape(n).to(torch.uint8).contiguous()
+    lib = _lib.load()
+    xmaps = min(nrow, n)
+    pad = 0 if n == 1 else padding
+    hg, wg = -(-n // xmaps) * (r + pad) + pad, xmaps * (r + pad) + pad
+    out = torch.empty((hg, wg, 3), dtype=torch.uint8, device=images.device)
+    points = torch.empty((n, p, 2), dtype=torch.float32, device=images.device)
+    ws_bytes = lib.gg_splat_composite_grid_workspace(1, n, r, int(alpha_channel is not None))
+    ws = torch.empty(max(1, ws_bytes // 4), dtype=torch.float32, device=images.device)
+    rc = lib.gg_splat_lookup_composite_grid(out.data_ptr(), points.data_ptr(), ws.data_ptr(), ws_bytes, images.data_ptr(),
+                                            grid.data_ptr(), query.data_ptr(), _lib.ptr(flip), colors.data_ptr(),
+                                            _lib.ptr(alpha_channel), float(sigma), float(opacity), n, p, query.size(0), 3, r,
+                                            grid.size(1), grid.size(2), int(nrow), int(padding), counts[0], counts[1],
+                                            _lib.stream())
+    _lib.check(rc, "gg_splat_lookup_composite_grid")
+    return out, points

@@ -121,6 +121,14 @@ class SimilarityHead(nn.Module):
         return out, grid, matrix, oob
 
 
+def resize_grid(flow, output_resolution):
+    """The sampling grid at output_resolution: resizing the grid beats resizing pixels (scale 1 is the identity)."""
+    if output_resolution == flow.size(2):
+        return flow
+    return F.interpolate(flow.permute(0, 3, 1, 2), scale_factor=output_resolution / flow.size(2),
+                         mode="bilinear").permute(0, 2, 3, 1)
+
+
 class FlowHead(nn.Module):
     """Regresses a dense sampling grid: low-res residual flow + RAFT-style convex upsampling mask."""
 
@@ -204,9 +212,7 @@ class FlowHead(nn.Module):
             img_size = torch.Size([img.size(0) * split, flow.size(1), flow.size(2)])
         else:
             img_size = torch.Size([img.size(0) * split, img.size(1), output_resolution, output_resolution])
-            if output_resolution != flow.size(2):  # resizing the grid beats resizing pixels (scale 1 is the identity)
-                flow = F.interpolate(flow.permute(0, 3, 1, 2), scale_factor=output_resolution / flow.size(2),
-                                     mode="bilinear").permute(0, 2, 3, 1)
+            flow = resize_grid(flow, output_resolution)
         if stop_grad:
             flow = flow.detach() + 0 * flow
         if split > 1:

@@ -10,7 +10,7 @@ import torch.nn as nn
 from ..opset import cuda_ops
 from ..splat2d.blend import BLEND_PRESETS
 from ..stylegan2.networks import ConvLayer, EqualLinear, ResBlock, channel_table
-from .heads import FlowHead, SimilarityHead
+from .heads import FlowHead, SimilarityHead, resize_grid
 from .sampling import BilinearDownsample
 
 
@@ -466,6 +466,35 @@ class ComposedSTN(nn.Module):
         if pointsB is not None:
             return imgA, imgB, pointsA, pointsB_out, pick
         return imgA, imgB, pointsA, pick
+
+    def congeal_and_grid(self, input_img, infer_flip=True, output_resolution=None, iters=1, padding_mode="border",
+                         warp_policy="cartesian"):
+        """Everything propagate_to_images reads from the STN (reference applications/propagate_to_images.py:44-78, which
+        runs it on 4N images: determine_flips' forward_with_flip (2N), t(reals_flipped) (N) and uncongeal_points (N)), from
+        ONE forward.  infer_flip: the forward runs over cat([x, flip(x)]) (2N images) and each image keeps the variant
+        with the smoother residual flow, by the op set's tv_per_sample and argmin as match_flows decides (a tie keeps x,
+        as forward_with_flip does).  Otherwise input_img (already flipped by the caller, e.g. by a cluster classifier)
+        runs once (N images) with warp_policy.  The forward samples at the flow size; at another output_resolution the
+        congealed image is sampled again on the grid resized as the flow head resizes it (heads.py), with no second
+        forward.  -> (flip (N,) bool or None, the congealed images (N, C, R, R) at output_resolution (None: the flow
+        size), the sampling grid (N, F, F, 2) at the flow size: the grid uncongeal_points(output_resolution=None) reads)."""
+        if not self.is_flow or not isinstance(self.stns[-1].warp_head, FlowHead):
+            raise ValueError("congeal_and_grid needs a ComposedSTN whose last stage is a flow")
+        if infer_flip and self.num_heads > 1:
+            raise ValueError("congeal_and_grid: a clustering STN takes its flips from the cluster classifier")
+        n = input_img.size(0)
+        x = torch.cat([input_img, input_img.flip(3,)], 0) if infer_flip else input_img
+        out, grid, delta = self.forward(x, return_warp=True, return_flow=True, iters=iters, padding_mode=padding_mode,
+                                        warp_policy=warp_policy)
+        flip = None
+        if infer_flip:
+            tv = self.ops.tv_per_sample(delta)
+            flip = torch.stack(tv.chunk(2), 0).argmin(dim=0).bool()
+            rows = torch.arange(n, device=x.device) + n * flip.long()
+            out, grid, x = out[rows], grid[rows], x[rows]
+        if output_resolution is not None and output_resolution != grid.size(2):
+            out = self.stns[-1].warp_head.warper(x, resize_grid(grid, output_resolution), padding_mode=padding_mode)
+        return flip, out, grid
 
     def _matrix_flow_grid(self, input_img, iters=1, **stn_forward_kwargs):
         """forward(input_img) of a similarity -> flow STN, returning what point transfer reads from it: the similarity

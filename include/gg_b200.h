@@ -259,6 +259,28 @@ GG_API int gg_splat_composite_grid(unsigned char* out, void* workspace, int64_t 
                                    int colors_n, int alpha_n, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * gg_splat_lookup_composite_grid -- a dense label or edit put on real images (reference
+ *   applications/propagate_to_images.py:62-73): gg_splat_composite_grid for one grid (T = 1) whose points are looked up
+ *   first.  For image n and point p:
+ *       q = query[query_n == 1 ? 0 : n, p]                              (normalised congealed-frame coordinates)
+ *       x, y = unnormalize(grid_sample(grid[n], q, 'border'), R, R)     (uncongeal_points, as gg_splat2d_lookup_forward:
+ *                                                                        k = (R - 1) / R, m = R - 1)
+ *       x = (R - 1) - x where flip[n]                                   (the point lands on the unflipped image)
+ *   then the splats, composite and grid of gg_splat_composite_grid at (x, y), whose layout and bytes it shares.
+ *   out (Hg, Wg, 3) uint8; points_out (N, P, 2) fp32 or NULL: the final pixel coordinates (the dense correspondences);
+ *   images (N, 3, R, R) fp32; grid (N, grid_h, grid_w, 2) fp32; query (query_n, P, 2) fp32; flip (N,) bytes or NULL
+ *   (no image flipped); colors (colors_n, P, 3), alpha (alpha_n, P, 1) or NULL.  query, grid and points_out 8-byte aligned.
+ *   P == 0: grid, query, colors and workspace may be NULL, and out is images2grid of the images.  C must be 3.
+ *   `workspace`: 16-byte aligned, at least gg_splat_composite_grid_workspace(1, N, R, alpha != NULL) bytes.
+ *   Arguments are validated before any device work (GG_ERR_BAD_ARG).
+ * ---------------------------------------------------------------------------------------------- */
+GG_API int gg_splat_lookup_composite_grid(unsigned char* out, float* points_out, void* workspace, int64_t workspace_bytes,
+                                          const float* images, const float* grid, const float* query,
+                                          const unsigned char* flip, const float* colors, const float* alpha, float sigma,
+                                          float opacity, int64_t N, int64_t P, int query_n, int C, int R, int grid_h,
+                                          int grid_w, int nrow, int padding, int colors_n, int alpha_n, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * The STN's sampling in ONE pass (north_star: "antialiased bilinear grid_sample fused with flow-compose in one pass").
  * The sampling grid is generated per output pixel from the head's raw outputs instead of being read from memory:
  *   mode 1  SimilarityHead (reference warping_heads.py:120-136): grid = F.affine_grid(theta (N, 2, 3), align_corners=False)

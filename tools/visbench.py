@@ -13,7 +13,12 @@ composition (oracle.vis.nearest_neighbor_within_patch on the device).
 Label propagation, N = 4, 512^2, 2 x 240 frames, a 256^2 label (65 536 points) at sigma 1.2: splat_composite_grid over all
 480 frames against the reference formulation (visualize_label_propagation: chunks of 100 (frame, image) pairs, two
 splat2d, the composite, .cpu(), then images2grid per frame on the host), timed over --label-chunks chunks and given per
-frame.  --labels-only runs this section alone.  Needs a CUDA device.
+frame.  --labels-only runs this section alone.
+--propagate runs only the edits-on-real-images comparison at 512^2, sigma 1.3, for N = 9 (the script's usual
+--dset_indices count) and N = 50 images and labels of P = 25 233 and 403 533 points (BASELINE config 4): the reference
+composition on the mirror (determine_flips, t(flipped), uncongeal_points, the x mirror, splat_points, then make_grid and the
+uint8 cast of each grid on the host) against propagate_to_images, in ms per batch, with the STN forwards (images through
+the flow STN) and C-ABI launches of each.  Needs a CUDA device.
 """
 import argparse
 import os
@@ -62,13 +67,76 @@ def main():
     ap.add_argument("--n-mean", type=int, default=1000)
     ap.add_argument("--label-chunks", type=int, default=2)
     ap.add_argument("--labels-only", action="store_true")
+    ap.add_argument("--propagate", action="store_true")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("visbench: needs a CUDA device")
     print("card: %s" % _card())
+    if args.propagate:
+        propagate()
+        return
     label_propagation(args.label_chunks)
     if not args.labels_only:
         congealing(args)
+
+
+def propagate():
+    """propagate_to_images against the reference's make_visuals composition on the mirror."""
+    from torchvision.utils import make_grid
+    from gangealing_b200 import _lib
+    from gangealing_b200.evaluation import propagate_to_images
+    from gangealing_b200.evaluation.propagate import label_queries
+    dev, res, sigma, opacity = "cuda", 512, 1.3, 0.75
+    t = opset.fill_parameters(get_stn(["similarity", "flow"], flow_size=128, supersize=res, channel_multiplier=0.5).eval(),
+                              51, gain=0.6).to(dev)
+    ops = t.ops
+    seen = [0]
+    t.stns[-1].register_forward_hook(lambda m, inp, out: seen.__setitem__(0, seen[0] + inp[0].size(0)))
+    g = torch.Generator().manual_seed(0)
+
+    def host_grid(x, nrow):
+        grid = make_grid(x.cpu(), nrow=nrow, padding=3, pad_value=-1.0, normalize=True, value_range=(-1, 1))
+        return grid.mul(255).add_(0.5).clamp_(0, 255).permute(1, 2, 0).to(torch.uint8)
+
+    for n in (9, 50):
+        images = torch.nn.functional.interpolate(torch.randn(n, 3, 32, 32, generator=g), size=(res, res), mode="bilinear",
+                                                 align_corners=False).to(dev)
+        nrow = int(n ** 0.5)
+        for p in (25233, 403533):
+            side = int(p ** 0.5) + 1    # the label: P pixels of a side x side image at resolution = side
+            idx = torch.randperm(side * side, generator=g)[:p].sort().values
+            label = torch.stack([idx % side, idx // side], -1)
+            colors = (torch.rand(1, p, 3, generator=g) * 2 - 1).to(dev)
+            alpha = torch.rand(1, p, 1, generator=g).to(dev)
+
+            def reference():
+                flipped, flips, policy = V.determine_flips(t, None, images)
+                congealed = t(flipped, warp_policy=policy, output_resolution=res)
+                queries, _ = label_queries(label.to(dev), side, res)
+                pts = t.uncongeal_points(flipped, queries.expand(n, p, 2), warp_policy=policy)
+                pts[:, :, 0] = torch.where(flips.view(-1, 1), res - 1 - pts[:, :, 0], pts[:, :, 0])
+                out = V._splat_points(ops, images, pts, colors, alpha, sigma, opacity)
+                return [host_grid(x, nrow) for x in (images, congealed, out)]
+
+            def fused():
+                r = propagate_to_images(t, images, label, colors, alpha, sigma, opacity, resolution=side)
+                return [r["input_images"], r["congealed_images"], r["propagated"]]
+
+            row = []
+            for name, fn in (("reference", reference), ("propagate_to_images", fused)):
+                fn()
+                seen[0], calls = 0, _lib.CALLS
+                fn()
+                torch.cuda.synchronize()
+                fwd, launches = seen[0], _lib.CALLS - calls
+                start = time.perf_counter()
+                for _ in range(3):
+                    fn()
+                torch.cuda.synchronize()
+                row.append((name, (time.perf_counter() - start) / 3 * 1e3, fwd, launches))
+            print("propagate N %d, P %d, %d^2: " % (n, p, res) + "; ".join(
+                "%s %.1f ms per batch, %d STN images, %d C-ABI calls" % r for r in row) +
+                  "; speed-up %.2fx" % (row[0][1] / row[1][1]))
 
 
 def label_propagation(chunks):

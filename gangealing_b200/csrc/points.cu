@@ -10,6 +10,9 @@
 // (order-preserving bits of the distance << 32 | index): smaller distance wins, equal distances resolve to the smaller
 // index -- exactly argmin's rule.  The distance is evaluated with the reference's expanded expression and operation order
 // (separately rounded products, no FMA contraction), so near-ties resolve like the reference's.
+// Non-finite distances follow torch.argmin too: a NaN counts as smaller than any number and the first NaN wins (every NaN
+// packs to the smallest key, 0 in the high word, so the splits merge by index alone), and a point whose distances are all
+// +inf resolves to index 0 (each split starts from its first entry, so every point issues its atomicMin).
 #include "common.cuh"
 #include "points.cuh"
 
@@ -20,9 +23,13 @@ constexpr int kNNThreads = 256;
 constexpr int kNNTile = 1024;     // grid entries per shared-memory tile
 
 __device__ __forceinline__ unsigned order_bits(float f) {   // monotone map float -> unsigned (handles negative rounding noise)
+  if (f != f) return 0u;                                    // every NaN below -inf's key (0x007fffff): argmin's rule
   const unsigned u = __float_as_uint(f);
   return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
+
+// argmin's order: `d` replaces the best `bd` so far if it is smaller, or if it is the first NaN
+__device__ __forceinline__ bool argmin_better(float d, float bd) { return d < bd || (d != d && bd == bd); }
 
 __global__ void nn_init_kernel(unsigned long long* __restrict__ best, int64_t total) {
   const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -44,8 +51,8 @@ nn_argmin_kernel(unsigned long long* __restrict__ best, const float* __restrict_
     py = __ldg(points + (n * P + pt) * 2 + 1);
     pp = __fadd_rn(__fmul_rn(px, px), __fmul_rn(py, py));          // pts.pow(2).sum(-1)
   }
-  float bd = INFINITY;
-  int bi = 0x7fffffff;
+  float bd = INFINITY;   // with bi = e0: the split's first entry, unless an entry is smaller or NaN
+  int bi = e0;
   const float* g = grid + n * HW * 2;
   for (int t0 = e0; t0 < e1; t0 += kNNTile) {
     const int cnt = min(kNNTile, e1 - t0);
@@ -61,11 +68,11 @@ nn_argmin_kernel(unsigned long long* __restrict__ best, const float* __restrict_
       for (int i = 0; i < cnt; ++i) {
         const float sim = __fadd_rn(__fmul_rn(sgx[i], px), __fmul_rn(sgy[i], py));      // (g @ p)
         const float d = __fsub_rn(__fadd_rn(pp, sgg[i]), __fmul_rn(2.f, sim));         // |p|^2 + |g|^2 - 2 sim
-        if (d < bd) { bd = d; bi = t0 + i; }
+        if (argmin_better(d, bd)) { bd = d; bi = t0 + i; }
       }
     }
   }
-  if (pt < P && bi != 0x7fffffff) {
+  if (pt < P && e0 < e1) {
     const unsigned long long key = (static_cast<unsigned long long>(order_bits(bd)) << 32) | static_cast<unsigned>(bi);
     atomicMin(best + n * P + pt, key);
   }
@@ -81,6 +88,8 @@ __global__ void nn_unpack_kernel(int64_t* __restrict__ index, const unsigned lon
 // (:183-205), for all T frames of a stage in one launch: one thread per point, its patch centre carried in registers.
 // Frame t's grid is lerp(base, target, alphas[t]) (torch.lerp's formula, as warp.cu MODE 3), seen through pad_grid's
 // (H+2) x (W+2) linear-extrapolation ring; window positions beyond the ring are Unfold's zero padding, (0, 0) candidates.
+// The window's argmin follows torch.argmin as the search above does: the first NaN wins, an all-+inf window picks its first
+// candidate.
 __device__ __forceinline__ float lerp_aten(float a, float b, float w) {
   const float d = b - a;
   return (fabsf(w) < 0.5f) ? fmaf(w, d, a) : fmaf(-d, 1.f - w, b);
@@ -147,7 +156,7 @@ track_points_kernel(int64_t* __restrict__ track, int64_t* __restrict__ centers, 
         const float sim = __fadd_rn(__fmul_rn(g.x, px), __fmul_rn(g.y, py));
         const float gg = __fadd_rn(__fmul_rn(g.x, g.x), __fmul_rn(g.y, g.y));
         const float d = __fsub_rn(__fadd_rn(pp, gg), __fmul_rn(2.f, sim));
-        if (d < bd) { bd = d; bk = ky * patch + kx; }
+        if (argmin_better(d, bd)) { bd = d; bk = ky * patch + kx; }   // bk = 0 seeds the first candidate
       }
     }
     // unravel over (patch, patch) -> (kx, ky); offset (kx - r) + (H + 2)(ky - r); unravel over (H + 2, W + 2) (floor

@@ -468,6 +468,7 @@ GG_API int gg_tent_downsample_backward(float* grad_in, const float* grad_out, co
  *   gg_nn_argmin: reference spatial_transformer.py:655-668 (`congeal_points` of a flow STN): index[n, p] = argmin over the
  *     HW entries of grid (N, HW, 2) of |p|^2 + |g|^2 - 2 g.p (the reference's expanded form and rounding; first minimum
  *     wins) for points (N, P, 2).  No (N, H, W, P) distance tensor; `workspace` of gg_nn_argmin_workspace(N, P) bytes.
+ *     Non-finite distances follow torch.argmin: the first NaN wins, an all-+inf row gives 0; every index is in [0, HW).
  *   gg_splat2d_lookup_forward: reference spatial_transformer.py:141-157 (`uncongeal_points`: F.grid_sample of the sampling
  *     grid at the query points, 'border', align_corners=False; `unnormalize` :621-623) fused into gg_splat2d_forward's point
  *     load: query (N, P, 2) normalised congealed-frame coordinates, grid (N, grid_h, grid_w, 2); pixel coordinate =
@@ -482,7 +483,8 @@ GG_API int gg_nn_argmin(int64_t* index, void* workspace, const float* grid, cons
  * Frame t searches the patch x patch window around each point's centre of pad_grid(lerp(base, target, alphas[t])) -- the
  * (H+2) x (W+2) grid with the linear-extrapolation ring; window positions beyond it are Unfold's (0, 0) zero padding and
  * stay candidates -- with the expanded distance |p|^2 + |g|^2 - 2 g.p (separately rounded; first minimum in row-major
- * window order wins) and carries the result as the next frame's centre.  The result index is flat_centre + dx + (H+2) dy,
+ * window order wins, and as with torch.argmin the first NaN, or the first candidate of an all-+inf window) and carries the
+ * result as the next frame's centre.  The result index is flat_centre + dx + (H+2) dy,
  * unravelled over (H+2, W+2) with floor division (a window leaving the padded grid wraps around) and minus 1.
  *   track (T, N, P, 2) int64 (x, y) per frame; centers (N, P, 2) int64 IN: centres before frame 0 (each in [-1, H]; the
  *   caller validates), OUT: the last frame's result; points (N, P, 2) fp32 normalised; base / target (N, H, W, 2) fp32

@@ -1,7 +1,8 @@
 """Congealing visualisations (gangealing_b200.evaluation.visuals): the average-image animation, the average congealed image
 and the congealing animation with dense point tracking, against the reference fixture (oracle/make_golden_vis.py), the
-float64 oracle (oracle/vis.py) and the reference's per-frame composition; the lerped-grid sampler, its frame-mean kernel and
-the windowed point tracker against torch and float64; a 2-rank gloo run; the C ABI's argument checks."""
+float64 oracle (oracle/vis.py) and the reference's per-frame composition; the lerped-grid sampler and its frame-mean kernel
+against torch and float64; a 2-rank gloo run; the C ABI's argument checks.  The windowed point tracker's kernel is checked
+over its launch plan in test_points_family_gpu.py."""
 import pytest
 import torch
 
@@ -244,61 +245,6 @@ def test_mipmap_warp_lerp_mean_is_the_sequential_sum(case):
     bound = n * src.float().abs().max().item() * (1e-4 + (2.0 ** -8 if dtype == torch.bfloat16 else 0.0))
     print("case %d: |mean - float64| = %.2e (bound %.2e)" % (case, err, bound))
     assert err <= bound
-
-
-def _tracker_case(g, n, h, p):
-    base = torch.nn.functional.affine_grid(torch.eye(2, 3).unsqueeze(0).repeat(n, 1, 1), (n, 1, h, h), align_corners=False)
-    base = base + 0.02 * torch.randn(base.shape, generator=g)
-    theta = torch.eye(2, 3).unsqueeze(0) * 0.7
-    theta = theta.repeat(n, 1, 1)
-    theta[:, :, 2] = 0.25 * torch.randn(n, 2, generator=g)
-    target = torch.nn.functional.affine_grid(theta, (n, 1, h, h), align_corners=False) + 0.02 * torch.randn(n, h, h, 2, generator=g)
-    points = torch.rand(n, p, 2, generator=g) * 2.4 - 1.2
-    centers = torch.randint(-1, h + 1, (n, p, 2), generator=g)
-    centers[:, :4] = torch.tensor([[-1, -1], [h, h], [-1, h], [h, 0]])       # windows leave the padded grid
-    return base, target, points, centers
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("patch", [1, 9, 37])
-def test_track_points_lerp_vs_float64_oracle(patch):
-    """Every frame of every stage against the oracle's step from the kernel's own previous centres (two stages, centres
-    carried): equal, or a tie of the two candidates' float64 distances within 1e-6 relative."""
-    from gangealing_b200.splat2d import track_points_lerp
-    g = torch.Generator().manual_seed(300 + patch)
-    n, h, p, T = 3, 24, 300, 6
-    ties = 0
-    _, stage2, _, _ = _tracker_case(g, n, h, p)
-    base, target, points, centers = _tracker_case(g, n, h, p)
-    alphas = torch.rand(T, generator=g)
-    c = centers
-    for b, tg in ((base, target), (target, stage2)):     # two stages, the centres carried
-        track, c_out = track_points_lerp(b.to(DEV), tg.to(DEV), alphas.to(DEV), points.to(DEV), c.to(DEV), patch)
-        track = track.cpu()
-        prev = c
-        for t in range(T):
-            grid = b.double().lerp(tg.double(), alphas[t].double())
-            want = OV.nearest_neighbor_within_patch(grid, points.double(), prev, patch)
-            differ = (track[t] != want).any(-1)
-            if differ.any():
-                d = OV.window_distances(grid, points, prev, patch)
-                r = patch // 2
-                def k_of(pos):
-                    flat = (prev[..., 0] + 1) + (h + 2) * (prev[..., 1] + 1)
-                    out = (pos[..., 0] + 1) + (h + 2) * (pos[..., 1] + 1)
-                    off = out - flat
-                    dy = torch.div(off + r + (h + 2) * r, h + 2, rounding_mode="floor") - r
-                    dx = off - (h + 2) * dy
-                    return (dy + r) * patch + (dx + r)
-                dk = d.gather(2, k_of(track[t]).unsqueeze(-1)).squeeze(-1)
-                dw = d.gather(2, k_of(want).unsqueeze(-1)).squeeze(-1)
-                tie = (dk - dw).abs() <= 1e-6 * dw.abs().clamp_min(1e-12)
-                assert bool(tie[differ].all()), "frame %d: %d points differ without a tie" % (t, int((differ & ~tie).sum()))
-                ties += int(differ.sum())
-            prev = track[t]
-        assert torch.equal(c_out.cpu(), track[-1])
-        c = c_out.cpu()
-    print("patch %d: %d near-tie differences of %d" % (patch, ties, 2 * T * n * p))
 
 
 def _count_images(t):

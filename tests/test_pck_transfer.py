@@ -3,8 +3,9 @@
 CPU: the oracle (oracle/pck.py) and the mirror STN on the oracle op set against the reference's own match_flows,
 transfer_points, forward_with_flip and pck_transfer (tests/golden/pck_transfer.npz); the single-forward evaluator against
 the reference's 8N composition; a 2-rank gloo run; the C ABI's argument checks; the error behaviour.
-GPU: tv_per_sample against float64; pck_transfer_points against the float64 oracle on identical grids; pck_transfer end to
-end against the CPU oracle op set and the fixture; CUDA-graph replay and run-to-run bit equality.
+GPU: tv_per_sample against float64; pck_transfer end to end against the CPU oracle op set and the fixture; CUDA-graph
+replay and run-to-run bit equality.  The kernels of pck_transfer_points are checked stage by stage over their launch plans
+in test_points_family_gpu.py.
 
 Comparisons exempt near-ties by one rule (oracle.pck.*_near_ties): a nearest neighbour whose second-best float64 distance
 lies within the rounding band of the best, an error within 1e-4 px of a threshold (scaled up where the grids themselves
@@ -253,34 +254,6 @@ def _transfer_case(composed, b, p, seed, f=64, s=128):
         grid_dst = torch.roll(delta, 1, 0) + torch.nn.functional.affine_grid(torch.roll(m, 1, 0), (b, 1, f, f), align_corners=False)
         kw = dict(delta_src=delta.contiguous(), identity=ident, grid_dst=grid_dst.contiguous())
     return (pts, gt, vis, thresh, alphas, m, s), kw
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("composed", [True, False], ids=["composed", "similarity"])
-@pytest.mark.parametrize("bp", [(12, 1), (6, 300), (2, 17)], ids=lambda v: "B%dxP%d" % v)
-def test_pck_transfer_points_vs_float64_oracle(composed, bp):
-    """Identical grids and matrices on both sides.  Rows come as pairs (row i's destination is row i + 1's source, all
-    directions in one call); thresholds per row; visibility masks a quarter of the points."""
-    from gangealing_b200.evaluation.ops import pck_transfer_points
-    args, kw = _transfer_case(composed, *bp, seed=bp[0] * 1000 + bp[1] + composed)
-    c64, e64, nn64 = OP.pck_transfer_points_ref(*[a.double() if torch.is_tensor(a) else a for a in args],
-                                                **{k: v.double() for k, v in kw.items()})
-    dev = lambda a: a.to(DEV) if torch.is_tensor(a) else a
-    counts, est, nn = pck_transfer_points(*map(dev, args), **{k: v.to(DEV) for k, v in kw.items()})
-    exempt = torch.zeros(bp, dtype=torch.bool)
-    if composed:
-        q = OP.congeal_query_ref(args[0].double(), args[5].double(), args[6], True)
-        exempt = OP.nn_near_ties(kw["delta_src"].double() + kw["identity"].double(), q, 1e-6)
-        assert exempt.float().mean() <= 0.02
-        assert torch.equal(nn.cpu()[~exempt], nn64[~exempt])
-    assert_close(est.cpu()[~exempt], e64[~exempt], atol=1e-5 * args[6], what="estimated points")
-    loose = exempt | OP.threshold_near_ties(e64, args[1], args[3], args[4])
-    vis = args[2] != 0
-    slack = (loose & vis).sum()
-    assert ((counts.cpu() - c64).abs() <= slack).all(), (counts, c64, slack)
-    if slack == 0:
-        assert torch.equal(counts.cpu(), c64)
-    assert torch.equal(pck_transfer_points(*map(dev, args), **{k: v.to(DEV) for k, v in kw.items()})[0], counts)
 
 
 @pytest.mark.gpu

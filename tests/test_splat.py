@@ -1,6 +1,7 @@
 """splat2d: CPU sanity of the restatement; GPU parity against the restatement AND the reference kernel itself
 (oracle/_ref/libsplat_ref.so, compiled from the reference's splat_gpu_impl.cu by oracle/build_ref.py).  The scatter and
-normalise kernels are checked element by element against float64 over their routes in test_splat_family_gpu.py."""
+normalise kernels are checked element by element against float64 over their routes in test_splat_family_gpu.py, the
+nearest-neighbour search of the point-transfer path in test_points_family_gpu.py."""
 import math
 
 import pytest
@@ -108,34 +109,6 @@ def test_splat2d_argument_checks_and_call_site_contract():
 
 
 # ------------------------------------------------------------------------------------------------ point-transfer kernels
-@pytest.mark.gpu
-def test_nn_argmin_kernel_against_the_reference_formulation():
-    """congeal_points' brute-force search (spatial_transformer.py:655-668): the tiled argmin kernel against the reference's
-    expanded-distance tensor + argmin on the CPU -- EXACT indices wherever the two smallest distances are separated."""
-    from gangealing_b200.splat2d import nn_argmin
-    g = torch.Generator().manual_seed(8)
-    for n, h, w, p in [(2, 16, 16, 37), (1, 128, 128, 3000), (3, 24, 40, 1)]:
-        ys, xs = torch.meshgrid(torch.linspace(-1, 1, h), torch.linspace(-1, 1, w), indexing="ij")
-        grid = torch.stack([xs, ys], -1)[None].repeat(n, 1, 1, 1) + 0.05 * torch.randn(n, h, w, 2, generator=g)
-        pts = torch.rand(n, p, 2, generator=g) * 2 - 1
-        gg_ = grid.reshape(n, h, w, 1, 1, 2)
-        pp = pts.reshape(n, 1, 1, p, 2, 1)
-        sim = (gg_ @ pp)[..., 0, 0]
-        dist = (pp.pow(2).squeeze(-1).sum(dim=-1) + gg_.pow(2).sum(dim=-1).squeeze(-1) - 2 * sim).reshape(n, h * w, p)
-        expect = dist.argmin(dim=1)
-        got = nn_argmin(grid.to(DEV), pts.to(DEV)).cpu()
-        top2 = dist.topk(2, dim=1, largest=False).values
-        decided = (top2[:, 1] - top2[:, 0]) > 1e-6
-        assert decided.float().mean() > 0.95
-        assert torch.equal(got[decided], expect[decided])
-        # wherever the kernel disagrees on an undecided pair it still picked a (numerically) minimal entry
-        picked = dist.gather(1, got[:, None, :]).squeeze(1)
-        assert torch.all(picked <= top2[:, 0] + 1e-5)
-    # exact duplicates: the first index wins, like argmin
-    grid = torch.zeros(1, 4, 4, 2)
-    assert int(nn_argmin(grid.to(DEV), torch.zeros(1, 1, 2, device=DEV))) == 0
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("sigma", [0.3, 1.3])
 def test_splat2d_lookup_fuses_uncongeal_points_into_the_splat(sigma):

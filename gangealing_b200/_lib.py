@@ -93,6 +93,8 @@ SIGNATURES = {
     "gg_flow_image_grid": (_I, [_P, _P, _P, _L, _I, _I, _I, _I, _P]),
     "gg_image_grid": (_I, [_P, _P, _P, _L, _I, _I, _I, _I, _P]),
     "gg_cluster_accumulate": (_I, [_P] * 5 + [_L, _I, _I, _I, _I, _I] + [_L] * 6 + [_I, _P]),
+    "gg_letterbox_plan": (_I, [_P, _L, _I, _I, _L, _P]),
+    "gg_letterbox": (_I, [_P, _P, _L, _P, _L, _P, _P, _P, _L, _I, _I, _P]),
 }
 
 _dll = None

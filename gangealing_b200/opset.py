@@ -29,6 +29,7 @@ def cuda_ops():
         from .evaluation import ops as _ev
         from .op import pca as _pca
         from .op import grids as _grids
+        from .op import letterbox as _letterbox
         _cached = types.SimpleNamespace(
             name="sm_90a",
             upfirdn2d=_op.upfirdn2d,
@@ -65,5 +66,6 @@ def cuda_ops():
             flow_image_grid=_grids.flow_image_grid,       # training visuals: colour-wheel flow images as a uint8 grid
             image_grid=_grids.image_grid,                 # ... min/max-normalised uint8 grid (per-image ranges)
             cluster_accumulate=_grids.cluster_accumulate,  # ... per-cluster sums of routed images, in order, on the device
+            letterbox=_letterbox.letterbox,               # dataset congealing: ragged uint8 -> Lanczos + edge pad, fp32
         )
     return _cached

@@ -54,6 +54,17 @@ def all_gather(tensor, cat=True):
     return torch.cat(out, 0) if cat else out
 
 
+def all_gatherv(tensor):
+    """Gather tensors whose first dimensions differ across ranks, concatenated in rank order (reference
+    distributed.py:103-122): the sizes are gathered first, every rank pads to the largest, the padding is dropped."""
+    if get_world_size() == 1:
+        return tensor
+    counts = all_gather(torch.tensor([tensor.size(0)], device=tensor.device)).tolist()
+    padded = torch.zeros((max(counts),) + tuple(tensor.shape[1:]), dtype=tensor.dtype, device=tensor.device)
+    padded[:tensor.size(0)] = tensor
+    return torch.cat([part[:c] for part, c in zip(all_gather(padded, cat=False), counts)], 0)
+
+
 def rank0_to_all(tensor):
     """Rank 0's value of `tensor` on every rank (reference distributed.py:134-137)."""
     return all_gather(tensor)[0]

@@ -612,6 +612,43 @@ GG_API int gg_cluster_accumulate(float* sums, int64_t* counts, float* keep, cons
                                  int64_t stride_head, int64_t stride_c, int64_t stride_h, int64_t stride_w, int n_keep,
                                  void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Dataset congealing's pre-processing, csrc/letterbox.cu: prepare_data.py:53-77 border_pad followed by
+ * applications/congeal_dataset.py:23-26 prepro, for a ragged batch of uint8 RGB images on the device.
+ *   images: the N images packed in one buffer of images_bytes bytes, image n (h, w, 3) uint8 HWC at byte info[n].offset.
+ *   out (N, 3, S, S) fp32: ((byte / 255) - 0.5) * 2, each operation rounded on its own.
+ *   resize = 1: Pillow's (12.2) Image.resize(LANCZOS) of 8-bit RGB to (S, round_half_even(S*h/w)) for h <= w, else
+ *     (round_half_even(S*w/h), S): separable fixed-point passes (22 fractional bits, sums from 1 << 21, clip to
+ *     [0, 255]) over a uint8 intermediate, horizontal first unless h > 100 * w and nh < h, an axis that keeps its size skipped;
+ *     coefficients in float64 as Pillow's precompute_coeffs.  Then np.pad(mode='edge') of the short axis by
+ *     (floor((S - n) / 2), the rest).
+ *   resize = 0: the edge pad only, S = max(h, w) for every image.
+ *   flip: N bytes (nonzero: write the horizontal mirror of the padded square) or NULL.
+ *   gg_letterbox_plan (host only, no device work): fills the derived fields of info_host[0..N) from (offset, h, w) and
+ *     returns the workspace bytes through workspace_bytes_host.  gg_letterbox re-derives them from info_host and refuses
+ *     a table that differs; the kernels read the same table from info (a device copy of info_host).
+ *   Three launches: coefficient tables, the first pass of images that need two, then the second pass (or the copy) with
+ *   the pad, the mirror and the normalisation.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct {
+  int64_t offset;          /* in: byte offset of the image in `images` */
+  int32_t h, w;            /* in: the image's size */
+  int32_t nh, nw;          /* resized size (h, w without resize) */
+  int32_t order;           /* passes: 0 none, 1 horizontal, 2 vertical, 3 horizontal then vertical, 4 vertical then
+                              horizontal */
+  int32_t ksize_h, ksize_v;  /* coefficients per output index of each pass (0: no such pass) */
+  int32_t reserved;
+  int64_t tmp_offset;      /* byte offset of the first pass's uint8 intermediate in the workspace (-1: none) */
+  int64_t coef_h, coef_v;  /* int32 offsets of the coefficient tables in the workspace (-1: none): per output index
+                              (first, count, ksize fixed-point weights) */
+} GGLetterboxImage;
+
+GG_API int gg_letterbox_plan(GGLetterboxImage* info_host, int64_t N, int S, int resize, int64_t images_bytes,
+                             int64_t* workspace_bytes_host);
+GG_API int gg_letterbox(float* out, void* workspace, int64_t workspace_bytes, const unsigned char* images,
+                        int64_t images_bytes, const GGLetterboxImage* info_host, const GGLetterboxImage* info,
+                        const unsigned char* flip, int64_t N, int S, int resize, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
